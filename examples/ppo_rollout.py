@@ -9,8 +9,11 @@ observations never leave the GPU.  The PPO update is plain torch; gradients are 
 minibatch and advantages are normalised with global statistics (gym_fx_b200.learner / gym_fx_b200.sharding).
 
     python examples/ppo_rollout.py --envs 4096 --horizon 32 --updates 5
+    python examples/ppo_rollout.py --envs 4096 --action-space continuous --updates 5 --eval-rollouts 2
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 examples/ppo_rollout.py --envs 4096
 
+--action-space continuous trains a Gaussian actor on the Box(-1, 1) action (thresholded to hold / long / short by the
+env); --eval-rollouts K runs K greedy rollouts (argmax / mean action) after training and reports their mean reward.
 Prints one JSON line: env-steps/s of the rollout phase (policy in the loop) and of the whole train loop.
 """
 from __future__ import annotations
@@ -37,7 +40,10 @@ def main():
     ap.add_argument("--minibatches", type=int, default=4)
     ap.add_argument("--workload", default="cfg4", help="bench.py workload shape (cfg4 = W=128, fixed SL/TP, sharpe)")
     ap.add_argument("--lr", type=float, default=3e-4)
+    ap.add_argument("--action-space", choices=("discrete", "continuous"), default="discrete")
+    ap.add_argument("--eval-rollouts", type=int, default=0, help="greedy rollouts after training")
     args = ap.parse_args()
+    continuous = args.action_space == "continuous"
 
     import bench
     from gym_fx_b200.learner import ActorCritic, ppo_update
@@ -55,14 +61,17 @@ def main():
         dist.init_process_group("nccl", device_id=dev)
 
     cfg, candles, minutes, N, D, _, desc = bench.build_workload(args.workload, args.envs)
+    if continuous:
+        cfg.action_mode = 1   # FX_ACTION_CONTINUOUS (action_space_mode "continuous")
+        desc += ", continuous actions"
     env = VecFxEnv(cfg, candles, minutes, device=dev)
     check_pair_alignment(N, cfg.num_pairs)
     H = args.horizon
-    env.reset(torch.as_tensor(shard_starts(N, rank, world, bench.T_BARS, (args.updates + 2) * H + 64, 256)))
+    env.reset(torch.as_tensor(shard_starts(N, rank, world, bench.T_BARS, (args.updates + args.eval_rollouts + 2) * H + 64, 256)))
 
     torch.backends.cuda.matmul.allow_tf32 = True
     torch.manual_seed(0)  # identical replicas on every rank
-    net = ActorCritic(D).to(dev)
+    net = ActorCritic(D, continuous=continuous).to(dev)
     opt = torch.optim.Adam(net.parameters(), lr=args.lr, eps=1e-5)
     policy = env.make_policy(net)
     buf = None
@@ -86,6 +95,17 @@ def main():
             t_upd += t2 - t1
         stats.update(mean_reward=float(buf["reward"].mean()), terminated_frac=float(buf["done"].float().mean()))
 
+    if args.eval_rollouts > 0:   # greedy evaluation of the trained policy, continuing from where training stopped
+        rew_sum = torch.zeros((), dtype=torch.float64, device=dev)
+        for _ in range(args.eval_rollouts):
+            buf = env.rollout(policy, H, buffers=buf, deterministic=True)
+            rew_sum += buf["reward"].double().mean()
+        ev = torch.stack([rew_sum / args.eval_rollouts])
+        if dist:
+            dist.all_reduce(ev, op=dist.ReduceOp.SUM)
+            ev /= world
+        stats["eval_mean_reward"] = float(ev[0])
+
     n_it = max(1, args.updates - 1)
     tt = torch.tensor([t_roll, t_upd], dtype=torch.float64, device=dev)
     if dist:
@@ -95,7 +115,8 @@ def main():
         steps = N * world * H * n_it
         print(json.dumps({
             "example": "ppo_rollout", "workload": desc, "n_gpus": world, "envs_per_gpu": N, "horizon": H,
-            "policy": f"MLP({D},256,256) actor-critic, fused wgmma kernel in the rollout, torch (tf32) in the update",
+            "policy": f"MLP({D},256,256) actor-critic ({args.action_space} actions), fused wgmma kernel in the rollout, "
+                      "torch (tf32) in the update",
             "rollout_env_steps_per_s": steps / max(t_roll, 1e-9), "rollout_us_per_step": t_roll / (H * n_it) * 1e6,
             "train_env_steps_per_s": steps / max(t_roll + t_upd, 1e-9), "update_s": t_upd / n_it, **stats}), flush=True)
     env.close()

@@ -30,7 +30,10 @@ EXPORTS = [
     "fxenv_reset", "fxenv_observe", "fxenv_step", "fxenv_step_many", "fxenv_step_host", "fxenv_get_info",
     "fxenv_state_bytes", "fxenv_get_state", "fxenv_set_state", "fxenv_launch_count", "fxenv_step_many_engine",
     "fxenv_policy_create", "fxenv_policy_set_weights", "fxenv_policy_destroy", "fxenv_rollout", "fxenv_policy_sync_timeouts",
+    "fxenv_rollout_ex",
 ]
+
+ROLLOUT_GREEDY = 1  # FXENV_ROLLOUT_GREEDY
 
 
 class FxEnvError(RuntimeError):
@@ -109,6 +112,7 @@ def load():
     L.fxenv_policy_set_weights.argtypes = [vp, C.POINTER(FxPolicyWeights), vp]
     L.fxenv_policy_destroy.argtypes = [vp]
     L.fxenv_rollout.argtypes = [vp, vp, C.POINTER(FxRollout), vp]
+    L.fxenv_rollout_ex.argtypes = [vp, vp, C.POINTER(FxRollout), C.c_uint32, vp]
     L.fxenv_policy_sync_timeouts.argtypes = [vp]
     if L.fxenv_abi_version() != 2:
         raise FxEnvError("libfxenv.so ABI version mismatch")

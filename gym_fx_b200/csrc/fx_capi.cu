@@ -604,7 +604,8 @@ struct FxPolicy {
   CUtensorMap map_obs[2], map_w1, map_w2, map_h1;
   FxPolicyDev dev;
   bool has_weights = false;
-  struct { cudaGraphExec_t exec = nullptr; FxRollout io; } cached;
+  bool continuous = false;             // FX_ACTION_CONTINUOUS: Gaussian head, float32 actions (fx_policy_kernel<true>)
+  struct { cudaGraphExec_t exec = nullptr; FxRollout io; uint32_t flags = 0; } cached;
 };
 
 namespace {
@@ -639,9 +640,13 @@ int make_map(FxEnv* env, CUtensorMap* map, void* base, uint64_t rows, uint64_t c
 // the graph).  While one group's 128-row policy tiles occupy a few SMs, the other groups' env steps use the rest of the
 // device, and a group of ~2048 envs steps in a single wave instead of the two of a 4096-env launch.  More, smaller groups
 // do not pay: every group adds two kernel nodes per step to the graph, and a group's policy tiles need SMs of their own.
-cudaError_t enqueue_rollout(FxEnv* env, FxPolicy* pol, const FxRollout& io, cudaStream_t s) {
+cudaError_t enqueue_rollout(FxEnv* env, FxPolicy* pol, const FxRollout& io, uint32_t flags, cudaStream_t s) {
   const size_t N = (size_t)env->P.cfg.num_envs, D = (size_t)env->P.obs_dim;
   const int H = io.horizon, slots = io.obs_slots;
+  const bool greedy = (flags & FXENV_ROLLOUT_GREEDY) != 0;
+  const size_t noise_per_env = pol->continuous ? 1 : 3;  // N(0,1) draws / Gumbel(0,1) draws per env and step
+  // int32 or float32 actions: 4 bytes either way
+  uint32_t* const actions = static_cast<uint32_t*>(io.actions);
   static const int skip = [] { const char* v = getenv("FXENV_ROLLOUT_SKIP"); return v ? atoi(v) : 0; }();  // timing experiments:
                                                                           // 1 = no env steps, 2 = no policy evaluations
   // FXENV_TILE_SYNC=1: per-tile hand-over between the two kernels (FxTileSync) instead of whole-kernel dependencies.
@@ -673,14 +678,15 @@ cudaError_t enqueue_rollout(FxEnv* env, FxPolicy* pol, const FxRollout& io, cuda
       const bool last = (t == H);  // the bootstrap evaluation: value only
       if (!(skip & 2))
       e = fx_launch_policy(pol->map_obs[t & 1], pol->map_w1, pol->map_w2, pol->map_h1, pol->dev, (int)N, pol->k_pad,
-                           (!last && io.gumbel) ? io.gumbel + (size_t)t * N * 3 : nullptr, io.seed, (unsigned)t,
-                           last ? pol->scratch_act : io.actions + (size_t)t * N, last ? pol->scratch_logp : io.logp + (size_t)t * N,
-                           io.value + (size_t)t * N, sg, (int)e0, (int)e1, tile_sync);
+                           (!last && io.gumbel) ? io.gumbel + (size_t)t * N * noise_per_env : nullptr, io.seed, (unsigned)t,
+                           last ? static_cast<void*>(pol->scratch_act) : actions + (size_t)t * N,
+                           last ? pol->scratch_logp : io.logp + (size_t)t * N, io.value + (size_t)t * N, sg, (int)e0, (int)e1,
+                           tile_sync, pol->continuous, greedy);
       if (e != cudaSuccess) return e;
       if (last) break;
       const FxTileSync ts = {pol->dev.act_flag, pol->sync + pol->tiles, pol->dev.timeouts, t + 1};
       if (!(skip & 1))
-      e = fx_launch_step(env->P, io.actions + (size_t)t * N, io.obs + (size_t)((t + 1) % slots) * N * D, io.reward + (size_t)t * N,
+      e = fx_launch_step(env->P, actions + (size_t)t * N, io.obs + (size_t)((t + 1) % slots) * N * D, io.reward + (size_t)t * N,
                          nullptr, io.done + (size_t)t * N, sg, (int)e0, (int)e1, pol->obs16[(t + 1) & 1], pol->k_pad,
                          tile_sync ? &ts : nullptr);
       if (e != cudaSuccess) return e;
@@ -726,11 +732,13 @@ int fxenv_policy_sync_timeouts(FxPolicy* pol) {
 int fxenv_policy_create(FxEnv* env, FxPolicy** out) {
   if (!env || !out) return FXENV_E_INVALID;
   *out = nullptr;
-  if (env->P.cfg.action_mode != FX_ACTION_DISCRETE) return fail(env, FXENV_E_INVALID, "the fused policy samples discrete actions");
+  if (env->P.cfg.action_mode != FX_ACTION_DISCRETE && env->P.cfg.action_mode != FX_ACTION_CONTINUOUS)
+    return fail(env, FXENV_E_INVALID, "unknown action mode");
   DeviceGuard g(env->device);
   FxPolicy* pol = new (std::nothrow) FxPolicy();
   if (!pol) return fail(env, FXENV_E_NOMEM, "out of host memory");
   pol->env = env;
+  pol->continuous = env->P.cfg.action_mode == FX_ACTION_CONTINUOUS;
   const size_t N = (size_t)env->P.cfg.num_envs, D = (size_t)env->P.obs_dim;
   pol->k_pad = (int)((D + 63) / 64 * 64);
   const size_t KP = (size_t)pol->k_pad, Hd = FX_POLICY_HIDDEN;
@@ -779,9 +787,16 @@ int fxenv_policy_set_weights(FxPolicy* pol, const FxPolicyWeights* w, void* stre
   float* f = pol->fparams;
   FX_CUDA(env, cudaMemcpyAsync(f, w->b1, Hd * 4, cudaMemcpyDeviceToDevice, s));
   FX_CUDA(env, cudaMemcpyAsync(f + Hd, w->b2, Hd * 4, cudaMemcpyDeviceToDevice, s));
-  FX_CUDA(env, cudaMemcpyAsync(f + 2 * Hd, w->w_pi, 3 * Hd * 4, cudaMemcpyDeviceToDevice, s));
+  if (pol->continuous) {  // head rows {w_mu, 0, 0, w_v}, head bias {b_mu, log sigma, 0, b_v}
+    FX_CUDA(env, cudaMemcpyAsync(f + 2 * Hd, w->w_pi, Hd * 4, cudaMemcpyDeviceToDevice, s));
+    FX_CUDA(env, cudaMemsetAsync(f + 3 * Hd, 0, 2 * Hd * 4, s));
+    FX_CUDA(env, cudaMemcpyAsync(f + 6 * Hd, w->b_pi, 2 * 4, cudaMemcpyDeviceToDevice, s));
+    FX_CUDA(env, cudaMemsetAsync(f + 6 * Hd + 2, 0, 4, s));
+  } else {
+    FX_CUDA(env, cudaMemcpyAsync(f + 2 * Hd, w->w_pi, 3 * Hd * 4, cudaMemcpyDeviceToDevice, s));
+    FX_CUDA(env, cudaMemcpyAsync(f + 6 * Hd, w->b_pi, 3 * 4, cudaMemcpyDeviceToDevice, s));
+  }
   FX_CUDA(env, cudaMemcpyAsync(f + 5 * Hd, w->w_v, Hd * 4, cudaMemcpyDeviceToDevice, s));
-  FX_CUDA(env, cudaMemcpyAsync(f + 6 * Hd, w->b_pi, 3 * 4, cudaMemcpyDeviceToDevice, s));
   FX_CUDA(env, cudaMemcpyAsync(f + 6 * Hd + 3, w->b_v, 4, cudaMemcpyDeviceToDevice, s));
   env->launches += 2;
   pol->has_weights = true;
@@ -789,9 +804,14 @@ int fxenv_policy_set_weights(FxPolicy* pol, const FxPolicyWeights* w, void* stre
 }
 
 int fxenv_rollout(FxEnv* env, FxPolicy* pol, const FxRollout* io, void* stream_) {
+  return fxenv_rollout_ex(env, pol, io, 0u, stream_);
+}
+
+int fxenv_rollout_ex(FxEnv* env, FxPolicy* pol, const FxRollout* io, uint32_t flags, void* stream_) {
   int rc = require_ready(env, true);
   if (rc) return rc;
   if (!pol || !io || pol->env != env) return fail(env, FXENV_E_INVALID, "policy does not belong to this env");
+  if (flags & ~(uint32_t)FXENV_ROLLOUT_GREEDY) return fail(env, FXENV_E_INVALID, "unknown rollout flags");
   if (!pol->has_weights) return fail(env, FXENV_E_STATE, "fxenv_policy_set_weights has not been called");
   if (io->horizon < 1 || io->obs_slots < 2) return fail(env, FXENV_E_INVALID, "horizon must be >= 1 and obs_slots >= 2");
   if (!io->obs || !io->actions || !io->logp || !io->value || !io->reward || !io->done) return fail(env, FXENV_E_INVALID, "null I/O pointer");
@@ -801,15 +821,16 @@ int fxenv_rollout(FxEnv* env, FxPolicy* pol, const FxRollout* io, void* stream_)
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
   if (stream != nullptr) cudaStreamIsCapturing(stream, &cs);
   if (cs != cudaStreamCaptureStatusNone || stream == nullptr || (env->P.debug & 32)) {  // inside a capture / legacy stream: plain launches
-    FX_CUDA(env, enqueue_rollout(env, pol, *io, stream));
+    FX_CUDA(env, enqueue_rollout(env, pol, *io, flags, stream));
     env->launches += nl;
     return FXENV_OK;
   }
-  if (!pol->cached.exec || memcmp(&pol->cached.io, io, sizeof(FxRollout)) != 0) {
+  // the graph bakes in the buffers, the seed and the flags (greedy or sampling): any change re-captures it
+  if (!pol->cached.exec || memcmp(&pol->cached.io, io, sizeof(FxRollout)) != 0 || pol->cached.flags != flags) {
     if (pol->cached.exec) { cudaGraphExecDestroy(pol->cached.exec); pol->cached.exec = nullptr; }
     cudaGraph_t graph = nullptr;
     FX_CUDA(env, cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
-    cudaError_t e = enqueue_rollout(env, pol, *io, stream);
+    cudaError_t e = enqueue_rollout(env, pol, *io, flags, stream);
     cudaError_t e2 = cudaStreamEndCapture(stream, &graph);
     if (e != cudaSuccess) { if (graph) cudaGraphDestroy(graph); return cuda_fail(env, e, "capture: rollout"); }
     if (e2 != cudaSuccess) return cuda_fail(env, e2, "cudaStreamEndCapture");
@@ -817,6 +838,7 @@ int fxenv_rollout(FxEnv* env, FxPolicy* pol, const FxRollout* io, void* stream_)
     cudaGraphDestroy(graph);
     if (e != cudaSuccess) { pol->cached.exec = nullptr; return cuda_fail(env, e, "cudaGraphInstantiate"); }
     pol->cached.io = *io;
+    pol->cached.flags = flags;
   }
   FX_CUDA(env, cudaGraphLaunch(pol->cached.exec, stream));
   env->launches += nl;

@@ -7,6 +7,13 @@
 //     action = argmax(logits + gumbel)          Gumbel-max sample (noise supplied, or counter-based in-kernel)
 //     logp   = logits[action] - logsumexp(logits)
 //
+// Continuous action mode (FX_ACTION_CONTINUOUS, the template parameter CONT): head row 0 is the mean, rows 1 and 2 are
+// unused, and the fp32 head bias holds {b_mu, log sigma, 0, b_v} -- the state-independent Gaussian of PPO:
+//     mu = h2 . wmu + bmu,  action = mu + sigma * eps   eps ~ N(0, 1) (noise supplied, or Box-Muller in-kernel)
+//     logp = -eps^2 / 2 - log sigma - log(2 pi) / 2
+// The sample is neither clipped nor squashed: the env step thresholds it (fx_coerce_continuous).  Greedy evaluation
+// (launch argument, both modes): the argmax of the logits / the mean, no noise read or generated.
+//
 // Layer 1 ([N x 900] . [900 x 256]) and layer 2 are real contractions: Hopper warpgroup tensor-core MMAs (wgmma).  A
 // 128-env row tile is owned by a CLUSTER OF TWO CTAs, each computing 128 of the 256 hidden units of both layers: a CTA
 // alone would stream the whole obs tile and all of W1 and W2 from L2 per tile, and only N / 128 SMs would have a tile;
@@ -154,15 +161,21 @@ __device__ __forceinline__ void cluster_sync() {
   asm volatile("barrier.cluster.wait.acquire;" ::: "memory");
 }
 
+// log(2 pi) / 2
+constexpr float kHalfLog2Pi = 0.918938533204672742f;
+
 // (min 2 CTAs per SM only to cap the registers at 112: a policy CTA then fits next to the one-warp CTAs of an env step
 // that is still draining, so its prologue -- barrier init, parameter loads, the first weight tiles -- overlaps the
 // step's tail instead of waiting for whole SMs to empty)
+// CONT = false: discrete actions (int32, Gumbel-max over 3 logits; noise: float32 [num_envs][3] Gumbel(0,1)).
+// CONT = true:  continuous actions (float32, Gaussian; noise: float32 [num_envs] N(0,1)).
+template <bool CONT>
 __global__ void __launch_bounds__(kThreads, 2)
 fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_constant__ CUtensorMap map_w1,
                  const __grid_constant__ CUtensorMap map_w2, const __grid_constant__ CUtensorMap map_h1, const FxPolicyDev pol,
-                 const int num_envs, const int k_blocks1, const float* __restrict__ gumbel, const unsigned long long seed,
-                 const unsigned step, int32_t* __restrict__ action, float* __restrict__ logp, float* __restrict__ value,
-                 const int env_begin, const int tile_sync) {
+                 const int num_envs, const int k_blocks1, const float* __restrict__ noise, const unsigned long long seed,
+                 const unsigned step, void* __restrict__ action_, float* __restrict__ logp, float* __restrict__ value,
+                 const int env_begin, const int tile_sync, const int greedy) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   Barriers* bar = reinterpret_cast<Barriers*>(smem + kOffBar);
@@ -297,8 +310,10 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
       const float h = fast_tanh(d[i] + b2[k - n0]);
       float* a = ((i / 2) & 1) ? acc_hi : acc_lo;
       a[0] = fmaf(h, head_w[k], a[0]);
-      a[1] = fmaf(h, head_w[kHidden + k], a[1]);
-      a[2] = fmaf(h, head_w[2 * kHidden + k], a[2]);
+      if (!CONT) {  // (continuous: rows 1 and 2 are zero and unused)
+        a[1] = fmaf(h, head_w[kHidden + k], a[1]);
+        a[2] = fmaf(h, head_w[2 * kHidden + k], a[2]);
+      }
       a[3] = fmaf(h, head_w[3 * kHidden + k], a[3]);
     }
     // the four lanes of a row hold interleaved columns: a fixed butterfly, so the sum does not depend on timing
@@ -324,22 +339,39 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
         const float4 o = pol.head_part[env];
         const float* hb = bias + 2 * kHidden;
         // (rank 0's columns first, then rank 1's: a fixed order, so the result does not depend on timing)
-        const float l0 = (acc[0] + o.x) + hb[0], l1 = (acc[1] + o.y) + hb[1], l2 = (acc[2] + o.z) + hb[2];
-        float g0, g1, g2;
-        if (gumbel) { g0 = gumbel[(size_t)env * 3]; g1 = gumbel[(size_t)env * 3 + 1]; g2 = gumbel[(size_t)env * 3 + 2]; }
-        else {
-          g0 = -__logf(-__logf(hash_uniform(seed, step, env, 0)));
-          g1 = -__logf(-__logf(hash_uniform(seed, step, env, 1)));
-          g2 = -__logf(-__logf(hash_uniform(seed, step, env, 2)));
+        if (CONT) {
+          const float mu = (acc[0] + o.x) + hb[0], log_std = hb[1];
+          float eps = 0.f;  // greedy: the mean
+          if (!greedy) {
+            if (noise) eps = noise[env];
+            else {  // Box-Muller over two counter-based uniforms in (0, 1)
+              float sn, cs;
+              sincospif(2.f * hash_uniform(seed, step, env, 1), &sn, &cs);
+              eps = sqrtf(-2.f * logf(hash_uniform(seed, step, env, 0))) * cs;
+            }
+          }
+          reinterpret_cast<float*>(action_)[env] = fmaf(expf(log_std), eps, mu);
+          logp[env] = (-0.5f * eps * eps - log_std) - kHalfLog2Pi;
+        } else {
+          const float l0 = (acc[0] + o.x) + hb[0], l1 = (acc[1] + o.y) + hb[1], l2 = (acc[2] + o.z) + hb[2];
+          float g0 = 0.f, g1 = 0.f, g2 = 0.f;  // greedy: the argmax of the logits
+          if (!greedy) {
+            if (noise) { g0 = noise[(size_t)env * 3]; g1 = noise[(size_t)env * 3 + 1]; g2 = noise[(size_t)env * 3 + 2]; }
+            else {
+              g0 = -__logf(-__logf(hash_uniform(seed, step, env, 0)));
+              g1 = -__logf(-__logf(hash_uniform(seed, step, env, 1)));
+              g2 = -__logf(-__logf(hash_uniform(seed, step, env, 2)));
+            }
+          }
+          const float s0 = l0 + g0, s1 = l1 + g1, s2 = l2 + g2;
+          int a = 0; float best = s0;  // first maximum wins, like torch.argmax
+          if (s1 > best) { best = s1; a = 1; }
+          if (s2 > best) { best = s2; a = 2; }
+          const float mx = fmaxf(l0, fmaxf(l1, l2));
+          const float lse = mx + logf(expf(l0 - mx) + expf(l1 - mx) + expf(l2 - mx));
+          reinterpret_cast<int32_t*>(action_)[env] = a;
+          logp[env] = (a == 0 ? l0 : (a == 1 ? l1 : l2)) - lse;
         }
-        const float s0 = l0 + g0, s1 = l1 + g1, s2 = l2 + g2;
-        int a = 0; float best = s0;  // first maximum wins, like torch.argmax
-        if (s1 > best) { best = s1; a = 1; }
-        if (s2 > best) { best = s2; a = 2; }
-        const float mx = fmaxf(l0, fmaxf(l1, l2));
-        const float lse = mx + logf(expf(l0 - mx) + expf(l1 - mx) + expf(l2 - mx));
-        action[env] = a;
-        logp[env] = (a == 0 ? l0 : (a == 1 ? l1 : l2)) - lse;
         value[env] = (acc[3] + o.w) + hb[3];
       }
     }
@@ -376,13 +408,15 @@ cudaError_t fx_policy_pack(const float* src, uint16_t* dst, int rows, int cols, 
 size_t fx_policy_smem_bytes() { return kSmemBytes; }
 
 cudaError_t fx_policy_configure() {
-  return cudaFuncSetAttribute(fx_policy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+  cudaError_t e = cudaFuncSetAttribute(fx_policy_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(fx_policy_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes);
 }
 
 cudaError_t fx_launch_policy(const CUtensorMap& map_obs, const CUtensorMap& map_w1, const CUtensorMap& map_w2,
-                             const CUtensorMap& map_h1, const FxPolicyDev& pol, int num_envs, int k_pad, const float* gumbel,
-                             unsigned long long seed, unsigned step, int32_t* action, float* logp, float* value,
-                             cudaStream_t stream, int env_begin, int env_end, bool tile_sync) {
+                             const CUtensorMap& map_h1, const FxPolicyDev& pol, int num_envs, int k_pad, const float* noise,
+                             unsigned long long seed, unsigned step, void* action, float* logp, float* value,
+                             cudaStream_t stream, int env_begin, int env_end, bool tile_sync, bool continuous, bool greedy) {
   if (env_end < 0) env_end = num_envs;
   cudaLaunchConfig_t lc = {};
   lc.gridDim = dim3(2 * ((env_end - env_begin + kTileM - 1) / kTileM));  // one CTA pair per 128-env tile
@@ -396,6 +430,7 @@ cudaError_t fx_launch_policy(const CUtensorMap& map_obs, const CUtensorMap& map_
   at[1].val.clusterDim.x = 2; at[1].val.clusterDim.y = 1; at[1].val.clusterDim.z = 1;
   lc.attrs = at;
   lc.numAttrs = 2;
-  return cudaLaunchKernelEx(&lc, fx_policy_kernel, map_obs, map_w1, map_w2, map_h1, pol, env_end, k_pad / kBlockK, gumbel, seed,
-                            step, action, logp, value, env_begin, (tile_sync && pol.act_flag) ? 1 : 0);
+  return cudaLaunchKernelEx(&lc, continuous ? fx_policy_kernel<true> : fx_policy_kernel<false>, map_obs, map_w1, map_w2, map_h1,
+                            pol, env_end, k_pad / kBlockK, noise, seed, step, action, logp, value, env_begin,
+                            (tile_sync && pol.act_flag) ? 1 : 0, greedy ? 1 : 0);
 }

@@ -13,6 +13,7 @@ and are masked out of the advantage statistics and of the loss; `done[t]` cuts t
 """
 from __future__ import annotations
 
+import math
 from typing import Dict, Optional
 
 import torch
@@ -23,17 +24,36 @@ from .sharding import allreduce_mean_grads
 
 
 class ActorCritic(nn.Module):
-    """Shared-body actor-critic in the layout FusedPolicy.set_weights reads (body[0], body[2], pi, v)."""
+    """Shared-body actor-critic in the layout FusedPolicy.set_weights reads (body[0], body[2], pi, v).
+    continuous=True (action_space_mode "continuous"): a Gaussian actor, `pi` = Linear(hidden, 1) gives the mean and the
+    parameter `log_std` [1] the state-independent log sigma; forward() then returns (mean [B, 1], value)."""
 
-    def __init__(self, obs_dim: int, hidden: int = 256, n_actions: int = 3):
+    def __init__(self, obs_dim: int, hidden: int = 256, n_actions: int = 3, continuous: bool = False,
+                 init_log_std: float = 0.0):
         super().__init__()
         self.body = nn.Sequential(nn.Linear(obs_dim, hidden), nn.Tanh(), nn.Linear(hidden, hidden), nn.Tanh())
-        self.pi = nn.Linear(hidden, n_actions)
+        self.pi = nn.Linear(hidden, 1 if continuous else n_actions)
         self.v = nn.Linear(hidden, 1)
+        self.continuous = continuous
+        if continuous:
+            self.log_std = nn.Parameter(torch.full((1,), float(init_log_std)))
 
     def forward(self, obs):
         h = self.body(obs)
         return self.pi(h), self.v(h).squeeze(-1)
+
+
+HALF_LOG_2PI = 0.5 * math.log(2.0 * math.pi)
+
+
+def gaussian_log_prob(mean, log_std, x):
+    """log N(x; mean, exp(log_std)^2), elementwise."""
+    return -0.5 * ((x - mean) * torch.exp(-log_std)) ** 2 - log_std - HALF_LOG_2PI
+
+
+def gaussian_entropy(log_std):
+    """Entropy of N(., exp(log_std)^2): log sigma + (1 + log 2 pi) / 2."""
+    return log_std + 0.5 + HALF_LOG_2PI
 
 
 def gae(reward, value, done, prev_done, gamma: float = 0.99, lam: float = 0.95):
@@ -70,10 +90,12 @@ def ppo_update(net: ActorCritic, opt, buf: Dict[str, torch.Tensor], prev_done: t
                minibatches: int = 4, clip: float = 0.2, vf_coef: float = 0.5, ent_coef: float = 0.01, max_grad_norm: float = 0.5,
                gamma: float = 0.99, lam: float = 0.95, timers: Optional[dict] = None) -> Dict[str, float]:
     """One PPO update from a rollout buffer (VecFxEnv.rollout).  `timers`, if given, receives CUDA-event pairs around the
-    collectives under "allreduce" so that the caller can report their share of the update."""
+    collectives under "allreduce" so that the caller can report their share of the update.  Floating-point actions
+    (continuous action mode) are scored by the Gaussian actor of ActorCritic(continuous=True)."""
     obs, act, logp_old, val, rew, done = (buf[k] for k in ("obs", "actions", "logp", "value", "reward", "done"))
     H, N = rew.shape
     D = obs.shape[-1]
+    continuous = act.is_floating_point()
 
     def timed(fn):
         if timers is None:
@@ -90,7 +112,7 @@ def ppo_update(net: ActorCritic, opt, buf: Dict[str, torch.Tensor], prev_done: t
         m, s = timed(lambda: masked_global_mean_std(adv, valid, dist))
         adv = (adv - m) / s
     b_obs = obs[:H].reshape(H * N, D)
-    b_act, b_logp = act.reshape(-1).long(), logp_old.reshape(-1)
+    b_act, b_logp = (act.reshape(-1) if continuous else act.reshape(-1).long()), logp_old.reshape(-1)
     b_adv, b_ret, b_valid = adv.reshape(-1), ret.reshape(-1), valid.reshape(-1)
     params = [p for p in net.parameters()]
     mb = (H * N) // minibatches
@@ -102,13 +124,19 @@ def ppo_update(net: ActorCritic, opt, buf: Dict[str, torch.Tensor], prev_done: t
             w = b_valid[idx]
             wn = w.sum().clamp(min=1.0)
             logits, v = net(b_obs[idx])
-            lp = torch.log_softmax(logits, -1)
-            new_logp = lp.gather(1, b_act[idx, None]).squeeze(1)
+            if continuous:  # logits = the Gaussian mean [mb, 1]
+                new_logp = gaussian_log_prob(logits.squeeze(-1), net.log_std, b_act[idx])
+            else:
+                lp = torch.log_softmax(logits, -1)
+                new_logp = lp.gather(1, b_act[idx, None]).squeeze(1)
             ratio = torch.exp(new_logp - b_logp[idx])
             a = b_adv[idx]
             pg = -(torch.min(ratio * a, torch.clamp(ratio, 1 - clip, 1 + clip) * a) * w).sum() / wn
             vloss = (F.mse_loss(v, b_ret[idx], reduction="none") * w).sum() / wn
-            ent = (-(lp.exp() * lp).sum(-1) * w).sum() / wn
+            if continuous:
+                ent = (gaussian_entropy(net.log_std) * w).sum() / wn
+            else:
+                ent = (-(lp.exp() * lp).sum(-1) * w).sum() / wn
             loss = pg + vf_coef * vloss - ent_coef * ent
             opt.zero_grad(set_to_none=True)
             loss.backward()

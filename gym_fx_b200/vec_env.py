@@ -291,15 +291,19 @@ class VecFxEnv:
         return FusedPolicy(self, weights)
 
     def rollout(self, policy: "FusedPolicy", horizon: int, buffers: Optional[Dict[str, torch.Tensor]] = None,
-                gumbel: Optional[torch.Tensor] = None, seed: int = 0) -> Dict[str, torch.Tensor]:
+                gumbel: Optional[torch.Tensor] = None, seed: int = 0, noise: Optional[torch.Tensor] = None,
+                deterministic: bool = False) -> Dict[str, torch.Tensor]:
         """`horizon` closed-loop steps (policy -> sample -> env.step) from the current state, all on the device: the
         loop of the reference's driver (app/main.py:57-65) with a learned policy.  Returns / fills `buffers`:
-        obs [H+1, N, D] (obs[t] is what the policy saw at step t), actions int32 [H, N], logp [H, N], value [H+1, N]
-        (value[H] bootstraps), reward [H, N], done uint8 [H, N].  gumbel: optional float32 [H, N, 3] Gumbel(0,1) noise
-        (reproducible sampling); default: the kernel's counter-based generator seeded with `seed`."""
+        obs [H+1, N, D] (obs[t] is what the policy saw at step t), actions [H, N] (int32, or float32 in continuous mode),
+        logp [H, N], value [H+1, N] (value[H] bootstraps), reward [H, N], done uint8 [H, N].
+        Sampling noise for reproducible rollouts -- discrete mode: gumbel, float32 [H, N, 3] Gumbel(0,1); continuous
+        mode: noise, float32 [H, N] standard normal; default: the kernel's counter-based generator seeded with `seed`.
+        deterministic: greedy evaluation, the most likely action (argmax of the logits / the Gaussian mean)."""
         H, N, D, dev = int(horizon), self.num_envs, self.obs_dim, self.device
+        continuous = self.action_dtype == torch.float32
         b = buffers if buffers is not None else {}
-        want = {"obs": ((H + 1, N, D), torch.float32), "actions": ((H, N), torch.int32), "logp": ((H, N), torch.float32),
+        want = {"obs": ((H + 1, N, D), torch.float32), "actions": ((H, N), self.action_dtype), "logp": ((H, N), torch.float32),
                 "value": ((H + 1, N), torch.float32), "reward": ((H, N), torch.float32), "done": ((H, N), torch.uint8)}
         for k, (shape, dt) in want.items():
             if k not in b:
@@ -310,14 +314,22 @@ class VecFxEnv:
                 self._check("obs", b[k], dt, (int(b[k].shape[0]), N, D))
             else:
                 self._check(k, b[k], dt, shape)
+        if continuous and gumbel is not None:
+            raise ValueError("gumbel noise is for discrete action mode; continuous mode takes `noise` [H, N]")
+        if not continuous and noise is not None:
+            raise ValueError("noise is for continuous action mode; discrete mode takes `gumbel` [H, N, 3]")
         if gumbel is not None:
             self._check("gumbel", gumbel, torch.float32, (H, N, 3))
+        if noise is not None:
+            self._check("noise", noise, torch.float32, (H, N))
+        eps = noise if continuous else gumbel
         io = _native.FxRollout(H, int(b["obs"].shape[0]), b["obs"].data_ptr(), b["actions"].data_ptr(), b["logp"].data_ptr(),
                                b["value"].data_ptr(), b["reward"].data_ptr(), b["done"].data_ptr(),
-                               0 if gumbel is None else gumbel.data_ptr(), int(seed) & (2**64 - 1))
-        rc = self.L.fxenv_rollout(self._h, policy._p, C.byref(io), self._stream())
-        _native.check(self.L, self._h, rc, "fxenv_rollout")
-        policy._keep = (b, gumbel)
+                               0 if eps is None else eps.data_ptr(), int(seed) & (2**64 - 1))
+        flags = _native.ROLLOUT_GREEDY if deterministic else 0
+        rc = self.L.fxenv_rollout_ex(self._h, policy._p, C.byref(io), flags, self._stream())
+        _native.check(self.L, self._h, rc, "fxenv_rollout_ex")
+        policy._keep = (b, eps)
         return b
 
     def launch_count(self) -> int:
@@ -379,12 +391,15 @@ def _tensor_from_ptr(ptr: int, n: int, dtype: torch.dtype, device: torch.device)
 class FusedPolicy:
     """Device-resident actor-critic MLP(obs_dim, 256, 256) -> 3 logits + value, evaluated between env steps by the fused
     wgmma kernel (gym_fx_b200/csrc/fx_policy.cu).  `set_weights` takes float32 CUDA tensors in torch.nn.Linear layout
-    (or a module with .body[0], .body[2], .pi, .v like examples/ppo_rollout.py's ActorCritic)."""
+    (or a module with .body[0], .body[2], .pi, .v like gym_fx_b200.learner.ActorCritic).
+    In continuous action mode the actor is a Gaussian: `pi` is Linear(256, 1) (the mean) and a `log_std` tensor of shape
+    [1] (dict key "log_std", or the module's .log_std parameter) gives the state-independent log sigma."""
 
     HIDDEN = 256
 
     def __init__(self, env: VecFxEnv, weights=None):
         self.env = env
+        self.continuous = env.action_dtype == torch.float32
         self._p = C.c_void_p()
         rc = env.L.fxenv_policy_create(env._h, C.byref(self._p))
         _native.check(env.L, env._h, rc, "fxenv_policy_create")
@@ -405,8 +420,18 @@ class FusedPolicy:
             m = weights
             weights = {"w1": m.body[0].weight, "b1": m.body[0].bias, "w2": m.body[2].weight, "b2": m.body[2].bias,
                        "w_pi": m.pi.weight, "b_pi": m.pi.bias, "w_v": m.v.weight, "b_v": m.v.bias}
+            if self.continuous:
+                if getattr(m, "log_std", None) is None:
+                    raise ValueError("continuous action mode needs a log_std parameter of shape [1] on the module")
+                weights["log_std"] = m.log_std
         D, Hd = self.env.obs_dim, self.HIDDEN
-        shapes = {"w1": (Hd, D), "b1": (Hd,), "w2": (Hd, Hd), "b2": (Hd,), "w_pi": (3, Hd), "b_pi": (3,), "w_v": (Hd,), "b_v": (1,)}
+        n_pi = 1 if self.continuous else 3
+        shapes = {"w1": (Hd, D), "b1": (Hd,), "w2": (Hd, Hd), "b2": (Hd,), "w_pi": (n_pi, Hd), "b_pi": (n_pi,), "w_v": (Hd,),
+                  "b_v": (1,)}
+        if self.continuous:
+            if "log_std" not in weights:
+                raise ValueError("continuous action mode needs weights['log_std'] of shape [1]")
+            shapes["log_std"] = (1,)
         ts = {}
         for k, shape in shapes.items():
             t = weights[k].detach()
@@ -416,6 +441,8 @@ class FusedPolicy:
             if tuple(t.shape) != shape:
                 raise ValueError(f"{k} must have shape {shape}, got {tuple(t.shape)}")
             ts[k] = t
+        if self.continuous:  # FxPolicyWeights.b_pi in continuous mode: {b_mu, log sigma}
+            ts["b_pi"] = torch.cat([ts["b_pi"], ts.pop("log_std")])
         w = _native.FxPolicyWeights(*[ts[k].data_ptr() for k in ("w1", "b1", "w2", "b2", "w_pi", "b_pi", "w_v", "b_v")])
         rc = self.env.L.fxenv_policy_set_weights(self._p, C.byref(w), self.env._stream())
         _native.check(self.env.L, self.env._h, rc, "fxenv_policy_set_weights")

@@ -18,6 +18,8 @@
  *   fxenv_observe                  GymFxEnv._make_observation           app/env.py:226-242
  *   fxenv_get_info                 GymFxEnv._make_info                  app/env.py:244-254
  *   fxenv_get_state/set_state      (no counterpart: env snapshot, SURVEY 8f #4)
+ *   fxenv_rollout / fxenv_rollout_ex  the caller loop of app/main.py:57-65 with a learned policy (see below);
+ *                                  continuous actions are the Box(-1, 1, (1,)) of app/env.py:71-80, 187-204
  *
  * Conventions: every function returns 0 on success, <0 on error (see FXENV_E_*); fxenv_last_error() gives the
  * message.  No exceptions or aborts cross the ABI.  The library owns env state (device struct-of-arrays) behind
@@ -239,10 +241,16 @@ int64_t fxenv_launch_count(const FxEnv* env);
  * Replaces the caller loop of app/main.py:57-65 (`action = strategy.decide_action(obs, info, step); env.step(action)`)
  * for a learned actor-critic (BASELINE configs[3]: PPO MLP(256,256)): observation rows never leave the GPU, and the
  * policy is one fused tensor-core kernel per step (wgmma / TMA / clusters, gym_fx_b200/csrc/fx_policy.cu), chained to the
- * env step kernel by programmatic dependent launches.  Discrete action mode only.
+ * env step kernel by programmatic dependent launches.  The actor head follows the env's FxConfig.action_mode:
  *
- *   h1 = tanh(obs W1^T + b1), h2 = tanh(h1 W2^T + b2), logits = h2 Wpi^T + bpi (3), value = h2 wv + bv
- *   action = argmax(logits + Gumbel noise), logp = log_softmax(logits)[action]
+ *   h1 = tanh(obs W1^T + b1), h2 = tanh(h1 W2^T + b2), value = h2 wv + bv
+ *   FX_ACTION_DISCRETE:   logits = h2 Wpi^T + bpi (3)
+ *                         action = argmax(logits + Gumbel noise), logp = log_softmax(logits)[action]
+ *   FX_ACTION_CONTINUOUS: mu = h2 wmu + bmu, learned state-independent log sigma
+ *                         action = mu + sigma * eps, eps ~ N(0, 1), logp = -eps^2 / 2 - log sigma - log(2 pi) / 2
+ *                         (not clipped: the env step thresholds the raw value, app/env.py:187-204)
+ *   greedy (fxenv_rollout_ex, FXENV_ROLLOUT_GREEDY): action = argmax(logits) (first maximum) / mu, with the log-prob of
+ *                         that action (continuous: -log sigma - log(2 pi) / 2); no noise is read or generated.
  * The two hidden layers run in bfloat16 with float32 accumulation (the env step writes a bfloat16 copy of each row for
  * this purpose); biases, heads, sampling and log-prob in float32. */
 typedef struct FxPolicy FxPolicy;
@@ -253,8 +261,8 @@ typedef struct FxPolicyWeights {
   const float* b1;   /* [256] */
   const float* w2;   /* [256][256] */
   const float* b2;   /* [256] */
-  const float* w_pi; /* [3][256] */
-  const float* b_pi; /* [3] */
+  const float* w_pi; /* discrete: [3][256] (one row per action);  continuous: [1][256] (the mean) */
+  const float* b_pi; /* discrete: [3];                            continuous: [2] = {b_mu, log sigma} */
   const float* w_v;  /* [256] */
   const float* b_v;  /* [1] */
 } FxPolicyWeights;
@@ -267,22 +275,29 @@ typedef struct FxRollout {
   int32_t horizon;
   int32_t obs_slots;
   float* obs;           /* [obs_slots][num_envs][obs_dim] */
-  int32_t* actions;     /* [horizon][num_envs] */
+  void* actions;        /* [horizon][num_envs]: int32 (discrete) or float32 (continuous) */
   float* logp;          /* [horizon][num_envs] */
   float* value;         /* [horizon + 1][num_envs] */
   float* reward;        /* [horizon][num_envs] */
   uint8_t* done;        /* [horizon][num_envs] */
-  const float* gumbel;  /* [horizon][num_envs][3] Gumbel(0,1) noise, or NULL: counter-based generator from `seed` */
+  const float* gumbel;  /* sampling noise, or NULL: counter-based generator from `seed`.  Discrete: [horizon][num_envs][3]
+                         * Gumbel(0,1); continuous: [horizon][num_envs] standard normal.  Unused by greedy rollouts. */
   uint64_t seed;
 } FxRollout;
 
+/* fxenv_rollout_ex flags */
+#define FXENV_ROLLOUT_GREEDY 1u   /* evaluation: the most likely action (argmax of the logits / the mean), no sampling */
+
+/* Discrete or continuous, as FxConfig.action_mode. */
 int fxenv_policy_create(FxEnv* env, FxPolicy** out);
 /* Converts / copies the parameters into the policy's own device buffers (stream-ordered; call after every optimiser step). */
 int fxenv_policy_set_weights(FxPolicy* pol, const FxPolicyWeights* weights_dev, void* stream);
 int fxenv_policy_destroy(FxPolicy* pol);
 /* `horizon` closed-loop steps starting from the env's current state; everything is enqueued on `stream`
- * (2 * horizon + 2 kernels; the launch sequence is cached as a CUDA graph per buffer set). */
+ * (2 * horizon + 2 kernels; the launch sequence is cached as a CUDA graph per buffer set and flags).
+ * fxenv_rollout(...) is fxenv_rollout_ex(..., 0, ...); flags: FXENV_ROLLOUT_* (unknown bits are an error). */
 int fxenv_rollout(FxEnv* env, FxPolicy* pol, const FxRollout* io, void* stream);
+int fxenv_rollout_ex(FxEnv* env, FxPolicy* pol, const FxRollout* io, uint32_t flags, void* stream);
 /* Inside a rollout the policy kernel and the env-step kernel hand 128-env tiles to each other through flags in device
  * memory instead of whole-kernel dependencies; a poll that is never answered gives up after ~0.3 s instead of hanging
  * the device.  Returns how many polls of the LAST rollout gave up (0 unless something is broken; then that rollout's
