@@ -30,10 +30,11 @@ EXPORTS = [
     "fxenv_reset", "fxenv_observe", "fxenv_step", "fxenv_step_many", "fxenv_step_host", "fxenv_get_info",
     "fxenv_state_bytes", "fxenv_get_state", "fxenv_set_state", "fxenv_launch_count", "fxenv_step_many_engine",
     "fxenv_policy_create", "fxenv_policy_set_weights", "fxenv_policy_destroy", "fxenv_rollout", "fxenv_policy_sync_timeouts",
-    "fxenv_rollout_ex",
+    "fxenv_rollout_ex", "fxenv_policy_peek",
 ]
 
 ROLLOUT_GREEDY = 1  # FXENV_ROLLOUT_GREEDY
+PEEK_OBS16, PEEK_H1 = 0, 1  # FXENV_PEEK_*
 
 
 class FxEnvError(RuntimeError):
@@ -114,6 +115,8 @@ def load():
     L.fxenv_rollout.argtypes = [vp, vp, C.POINTER(FxRollout), vp]
     L.fxenv_rollout_ex.argtypes = [vp, vp, C.POINTER(FxRollout), C.c_uint32, vp]
     L.fxenv_policy_sync_timeouts.argtypes = [vp]
+    L.fxenv_policy_peek.restype = i64
+    L.fxenv_policy_peek.argtypes = [vp, i32, i32, vp, i64, vp]
     if L.fxenv_abi_version() != 2:
         raise FxEnvError("libfxenv.so ABI version mismatch")
     _lib = L

@@ -729,6 +729,27 @@ int fxenv_policy_sync_timeouts(FxPolicy* pol) {
   return (int)v;
 }
 
+int64_t fxenv_policy_peek(FxPolicy* pol, int what, int slot, void* dst, int64_t bytes, void* stream) {
+  if (!pol) return FXENV_E_INVALID;
+  FxEnv* env = pol->env;
+  const void* src = nullptr;
+  int64_t n = 0;
+  if (what == FXENV_PEEK_OBS16 && (slot == 0 || slot == 1)) {
+    src = pol->obs16[slot];
+    n = (int64_t)env->P.cfg.num_envs * pol->k_pad * 2;
+  } else if (what == FXENV_PEEK_H1 && slot == 0) {
+    src = pol->h1;
+    n = (int64_t)pol->tiles * FX_POLICY_TILE_M * FX_POLICY_HIDDEN * 2;
+  } else {
+    return fail(env, FXENV_E_INVALID, "fxenv_policy_peek: unknown buffer or slot");
+  }
+  if (!dst) return n;
+  if (bytes < n) return fail(env, FXENV_E_INVALID, "fxenv_policy_peek: destination too small");
+  DeviceGuard g(env->device);
+  FX_CUDA(env, cudaMemcpyAsync(dst, src, (size_t)n, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return n;
+}
+
 int fxenv_policy_create(FxEnv* env, FxPolicy** out) {
   if (!env || !out) return FXENV_E_INVALID;
   *out = nullptr;

@@ -415,6 +415,24 @@ class FusedPolicy:
             _native.check(self.env.L, self.env._h, rc, "fxenv_policy_sync_timeouts")
         return rc
 
+    def peek(self, what: str, slot: int = 0) -> torch.Tensor:
+        """Copy of an internal device buffer of the policy, for tests and debugging (fxenv_policy_peek), ordered on the
+        current stream.  what = "obs16": the bf16 observation copy of `slot` (0 or 1) that the kernel reads,
+        [num_envs, k_pad]; "h1": the layer-1 activations of the last evaluation, [num_envs rounded up to 128, 256]."""
+        code = {"obs16": _native.PEEK_OBS16, "h1": _native.PEEK_H1}.get(what)
+        if code is None:
+            raise ValueError(f"what must be 'obs16' or 'h1', got {what!r}")
+        L, s = self.env.L, self.env._stream()
+        n = int(L.fxenv_policy_peek(self._p, code, int(slot), None, 0, s))
+        if n < 0:
+            _native.check(L, self.env._h, n, "fxenv_policy_peek")
+        cols = self.HIDDEN if what == "h1" else (self.env.obs_dim + 63) // 64 * 64
+        out = torch.empty((n // (2 * cols), cols), dtype=torch.int16, device=self.env.device)
+        rc = int(L.fxenv_policy_peek(self._p, code, int(slot), out.data_ptr(), n, s))
+        if rc < 0:
+            _native.check(L, self.env._h, rc, "fxenv_policy_peek")
+        return out.view(torch.bfloat16)
+
     def set_weights(self, weights):
         if not isinstance(weights, dict):
             m = weights

@@ -304,6 +304,15 @@ int fxenv_rollout_ex(FxEnv* env, FxPolicy* pol, const FxRollout* io, uint32_t fl
  * results are invalid), or <0.  Synchronises the device. */
 int fxenv_policy_sync_timeouts(FxPolicy* pol);
 
+/* fxenv_policy_peek `what` */
+#define FXENV_PEEK_OBS16 0   /* slot 0 | 1: the bf16 observation copy the policy reads, [num_envs][k_pad] (k_pad = obs_dim
+                              * rounded up to a multiple of 64, zero pad columns); a rollout's step t reads slot t % 2 */
+#define FXENV_PEEK_H1 1      /* slot 0: the layer-1 activations of the last policy evaluation (after a rollout: the
+                              * bootstrap one), bf16 [num_envs rounded up to a multiple of 128][256] */
+/* Test / debugging aid: stream-ordered copy of an internal policy buffer into caller DEVICE memory `dst` of `bytes`
+ * bytes.  dst == NULL: returns the byte size needed.  Returns the bytes copied, or <0.  Reads only. */
+int64_t fxenv_policy_peek(FxPolicy* pol, int what, int slot, void* dst, int64_t bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -13,6 +13,7 @@ import torch
 import torch.nn as nn
 
 import scenarios as S
+from policy_ref import forward_ref
 from gym_fx_b200.config import lower_config
 from gym_fx_b200.synth import start_offsets, synth_candles, synth_minutes
 
@@ -39,15 +40,14 @@ def _env(N, W=128, strategy="direct_fixed_sltp", reward="pnl_reward", T=6000, **
 
 
 def _ref_forward(net, obs, emulate_bf16):
-    """-> logits [N,3], value [N] in fp32; emulate_bf16: the kernel's arithmetic contract."""
-    w1, b1, w2, b2 = net.body[0].weight, net.body[0].bias, net.body[2].weight, net.body[2].bias
+    """-> logits [N,3], value [N] in fp32; emulate_bf16: the kernel's arithmetic contract (policy_ref.forward_ref),
+    else the pure fp32 MLP."""
     if emulate_bf16:
-        r = lambda t: t.to(torch.bfloat16).to(torch.float32)
-        h1 = torch.tanh(r(obs).double() @ r(w1).double().T + b1.double()).float()
-        h2 = torch.tanh(r(h1).double() @ r(w2).double().T + b2.double()).float()
-    else:
-        h1 = torch.tanh(obs.double() @ w1.double().T + b1.double()).float()
-        h2 = torch.tanh(h1.double() @ w2.double().T + b2.double()).float()
+        r = forward_ref(net, obs)
+        return r["head"].float(), r["value"].float()
+    w1, b1, w2, b2 = net.body[0].weight, net.body[0].bias, net.body[2].weight, net.body[2].bias
+    h1 = torch.tanh(obs.double() @ w1.double().T + b1.double()).float()
+    h2 = torch.tanh(h1.double() @ w2.double().T + b2.double()).float()
     logits = (h2.double() @ net.pi.weight.double().T + net.pi.bias.double()).float()
     value = (h2.double() @ net.v.weight.double().T + net.v.bias.double()).float().squeeze(-1)
     return logits, value

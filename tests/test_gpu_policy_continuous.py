@@ -11,6 +11,7 @@ import pytest
 import torch
 
 import scenarios as S
+from policy_ref import forward_ref
 from gym_fx_b200.config import lower_config
 from gym_fx_b200.learner import ActorCritic
 from gym_fx_b200.synth import start_offsets, synth_candles, synth_minutes
@@ -34,14 +35,10 @@ def _env(N, W=128, strategy="direct_fixed_sltp", reward="pnl_reward", T=6000, co
 
 
 def _ref_forward(net, obs):
-    """-> actor head output [N, n] (logits, or the Gaussian mean with n = 1), value [N]: the kernel's bf16 contract."""
-    w1, b1, w2, b2 = net.body[0].weight, net.body[0].bias, net.body[2].weight, net.body[2].bias
-    r = lambda t: t.to(torch.bfloat16).to(torch.float32)
-    h1 = torch.tanh(r(obs).double() @ r(w1).double().T + b1.double()).float()
-    h2 = torch.tanh(r(h1).double() @ r(w2).double().T + b2.double()).float()
-    head = (h2.double() @ net.pi.weight.double().T + net.pi.bias.double()).float()
-    value = (h2.double() @ net.v.weight.double().T + net.v.bias.double()).float().squeeze(-1)
-    return head, value
+    """-> actor head output [N, n] (logits, or the Gaussian mean with n = 1), value [N]: the kernel's bf16 contract
+    (policy_ref.forward_ref)."""
+    r = forward_ref(net, obs)
+    return r["head"].float(), r["value"].float()
 
 
 def _gaussian_net(D, log_std):
