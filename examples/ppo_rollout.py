@@ -10,10 +10,17 @@ minibatch and advantages are normalised with global statistics (gym_fx_b200.lear
 
     python examples/ppo_rollout.py --envs 4096 --horizon 32 --updates 5
     python examples/ppo_rollout.py --envs 4096 --action-space continuous --updates 5 --eval-rollouts 2
+    python examples/ppo_rollout.py --envs 4096 --episode-bars 500 --holdout-frac 0.2 --eval-rollouts 2
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 examples/ppo_rollout.py --envs 4096
 
 --action-space continuous trains a Gaussian actor on the Box(-1, 1) action (thresholded to hold / long / short by the
 env); --eval-rollouts K runs K greedy rollouts (argmax / mean action) after training and reports their mean reward.
+--episode-bars B cuts the table into episodes of B bars (auto-reset starts the next one).  --holdout-frac F keeps the
+last F of every table out of training: training episodes start at bars drawn from the first 1 - F (every auto-reset
+draws a new one, VecFxEnv.set_episode_starts), and the greedy evaluation resets every env into the held-out tail.  The
+episode records (VecFxEnv.episode_stats) then give, for training and for evaluation, the episodes finished and the mean
+total return and maximum drawdown of each env's last finished episode (the reset into the tail, and one after the
+evaluation, record the episodes they cut short).
 Prints one JSON line: env-steps/s of the rollout phase (policy in the loop) and of the whole train loop.
 """
 from __future__ import annotations
@@ -42,8 +49,15 @@ def main():
     ap.add_argument("--lr", type=float, default=3e-4)
     ap.add_argument("--action-space", choices=("discrete", "continuous"), default="discrete")
     ap.add_argument("--eval-rollouts", type=int, default=0, help="greedy rollouts after training")
+    ap.add_argument("--episode-bars", type=int, default=0, help="bars per episode (0: an episode runs to the end of the table)")
+    ap.add_argument("--holdout-frac", type=float, default=0.0,
+                    help="fraction of every table held out of training for the greedy evaluation (needs --episode-bars)")
     args = ap.parse_args()
     continuous = args.action_space == "continuous"
+    if not 0.0 <= args.holdout_frac < 1.0:
+        ap.error("--holdout-frac must be in [0, 1)")
+    if args.holdout_frac > 0.0 and args.episode_bars <= 0:
+        ap.error("--holdout-frac needs --episode-bars (an episode must fit inside its part of the table)")
 
     import bench
     from gym_fx_b200.learner import ActorCritic, ppo_update
@@ -64,10 +78,22 @@ def main():
     if continuous:
         cfg.action_mode = 1   # FX_ACTION_CONTINUOUS (action_space_mode "continuous")
         desc += ", continuous actions"
+    if args.episode_bars > 0:
+        cfg.episode_bars = args.episode_bars
+        desc += f", episodes of {args.episode_bars} bars"
     env = VecFxEnv(cfg, candles, minutes, device=dev)
     check_pair_alignment(N, cfg.num_pairs)
     H = args.horizon
-    env.reset(torch.as_tensor(shard_starts(N, rank, world, bench.T_BARS, (args.updates + args.eval_rollouts + 2) * H + 64, 256)))
+    T, L = bench.T_BARS, args.episode_bars
+    split = int(T * (1.0 - args.holdout_frac))       # training bars [0, split), held-out bars [split, T)
+    if args.holdout_frac > 0.0:
+        if split - L < 0 or T - L < split:
+            ap.error("--episode-bars is too long for the training part or the held-out part of the table")
+        desc += f", last {args.holdout_frac:g} of the table held out"
+        env.set_episode_starts(0, split - L, seed=0x5EED0000 + rank)   # a window [start, start + L) inside training
+        env.reset()
+    else:
+        env.reset(torch.as_tensor(shard_starts(N, rank, world, T, (args.updates + args.eval_rollouts + 2) * H + 64, 256)))
 
     torch.backends.cuda.matmul.allow_tf32 = True
     torch.manual_seed(0)  # identical replicas on every rank
@@ -95,7 +121,26 @@ def main():
             t_upd += t2 - t1
         stats.update(mean_reward=float(buf["reward"].mean()), terminated_frac=float(buf["done"].float().mean()))
 
-    if args.eval_rollouts > 0:   # greedy evaluation of the trained policy, continuing from where training stopped
+    def episode_report(prefix, done_before):
+        """Episodes finished since `done_before` and the mean total return / max drawdown of each env's last finished one
+        (envs without one are left out), summed / averaged over the ranks."""
+        ep = env.episode_stats()
+        new = (ep["episodes_done"] - done_before).double()
+        has = (new > 0).double()
+        v = torch.stack([new.sum(), has.sum(), (ep["total_return"] * has).sum(), (ep["max_drawdown_pct"] * has).sum()])
+        if dist:
+            dist.all_reduce(v, op=dist.ReduceOp.SUM)
+        n = max(float(v[1]), 1.0)
+        return {f"{prefix}_episodes": int(v[0]), f"{prefix}_mean_total_return": float(v[2]) / n if v[1] > 0 else None,
+                f"{prefix}_mean_max_drawdown_pct": float(v[3]) / n if v[1] > 0 else None}
+
+    holdout = args.holdout_frac > 0.0
+    if holdout:   # every env into a fresh episode in the held-out tail; the reset records the training episodes it ends
+        env.set_episode_starts(split, T - L, seed=0xE7A10000 + rank)
+        env.reset()
+        stats.update(episode_report("train", torch.zeros_like(env.episode_stats()["episodes_done"])))
+        done0 = env.episode_stats()["episodes_done"].clone()
+    if args.eval_rollouts > 0:   # greedy evaluation of the trained policy (held out: from the fresh episodes)
         rew_sum = torch.zeros((), dtype=torch.float64, device=dev)
         for _ in range(args.eval_rollouts):
             buf = env.rollout(policy, H, buffers=buf, deterministic=True)
@@ -105,6 +150,9 @@ def main():
             dist.all_reduce(ev, op=dist.ReduceOp.SUM)
             ev /= world
         stats["eval_mean_reward"] = float(ev[0])
+        if holdout:
+            env.reset()          # records the evaluation episodes still running
+            stats.update(episode_report("eval", done0))
 
     n_it = max(1, args.updates - 1)
     tt = torch.tensor([t_roll, t_upd], dtype=torch.float64, device=dev)

@@ -30,7 +30,7 @@ EXPORTS = [
     "fxenv_reset", "fxenv_observe", "fxenv_step", "fxenv_step_many", "fxenv_step_host", "fxenv_get_info",
     "fxenv_state_bytes", "fxenv_get_state", "fxenv_set_state", "fxenv_launch_count", "fxenv_step_many_engine",
     "fxenv_policy_create", "fxenv_policy_set_weights", "fxenv_policy_destroy", "fxenv_rollout", "fxenv_policy_sync_timeouts",
-    "fxenv_rollout_ex", "fxenv_policy_peek",
+    "fxenv_rollout_ex", "fxenv_policy_peek", "fxenv_set_reset_starts", "fxenv_get_episode_info",
 ]
 
 ROLLOUT_GREEDY = 1  # FXENV_ROLLOUT_GREEDY
@@ -49,6 +49,15 @@ class FxInfoPtrs(C.Structure):
 RUN_STATS = 12  # FXENV_RUN_STATS
 RS = {"dd_maxvalue": 0, "dd_max_money": 1, "dd_max_pct": 2, "tr_pnl": 3, "tr_comm": 4, "tr_price": 5, "pnl_net": 6,
       "pnl_sq": 7, "spare": 8, "opened": 9, "won": 10, "lost": 11}  # FXENV_RS_*
+
+
+class FxEpisodePtrs(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("start", "episodes_done", "last_episode")]
+
+
+EPISODE_STATS = 14  # FXENV_EPISODE_STATS
+EP = {"start": 0, "bars": 1, "equity": 2, "commission": 3, "end_flags": 4, "dd_max_pct": 5, "dd_max_money": 6,
+      "pnl_net": 7, "pnl_sq": 8, "opened": 9, "closed": 10, "won": 11, "lost": 12, "index": 13}  # FXENV_EP_*
 
 
 INFO_DTYPES = {
@@ -117,6 +126,8 @@ def load():
     L.fxenv_policy_sync_timeouts.argtypes = [vp]
     L.fxenv_policy_peek.restype = i64
     L.fxenv_policy_peek.argtypes = [vp, i32, i32, vp, i64, vp]
+    L.fxenv_set_reset_starts.argtypes = [vp, vp, vp, C.c_uint64]
+    L.fxenv_get_episode_info.argtypes = [vp, C.POINTER(FxEpisodePtrs)]
     if L.fxenv_abi_version() != 2:
         raise FxEnvError("libfxenv.so ABI version mismatch")
     _lib = L

@@ -217,6 +217,8 @@ int fxenv_create(const FxConfig* cfg, FxEnv** out) {
   o_p0 = plan.add(N * capP * 8);
   o_p1 = plan.add(N * capP * 8);
   o_sz = plan.add(N * capP * 8);
+  const size_t o_ep_lo = plan.add(N * 8), o_ep_span = plan.add(N * 8), o_ep_seed = plan.add(8);
+  const size_t o_ep_begun = plan.add(N * 4), o_ep_done = plan.add(N * 4), o_ep_last = plan.add(N * FXENV_EPISODE_STATS * 8);
   env->slab_bytes = plan.bytes;
   ce = cudaMalloc(&env->slab, plan.bytes);
   if (ce != cudaSuccess) { fxenv_destroy(env); return cuda_fail(nullptr, ce, "cudaMalloc(state slab)"); }
@@ -242,6 +244,12 @@ int fxenv_create(const FxConfig* cfg, FxEnv** out) {
   st.o_p0 = reinterpret_cast<double*>(b + o_p0);
   st.o_p1 = reinterpret_cast<double*>(b + o_p1);
   st.o_sz = reinterpret_cast<double*>(b + o_sz);
+  st.ep_lo = reinterpret_cast<int64_t*>(b + o_ep_lo);
+  st.ep_span = reinterpret_cast<uint64_t*>(b + o_ep_span);
+  st.ep_seed = reinterpret_cast<uint64_t*>(b + o_ep_seed);
+  st.ep_begun = reinterpret_cast<int32_t*>(b + o_ep_begun);
+  st.ep_done = reinterpret_cast<int32_t*>(b + o_ep_done);
+  st.ep_last = reinterpret_cast<double*>(b + o_ep_last);
   *out = env;
   return FXENV_OK;
 }
@@ -545,6 +553,46 @@ int fxenv_set_state(FxEnv* env, const void* buf_host, int64_t nbytes) {
 }
 
 int64_t fxenv_launch_count(const FxEnv* env) { return env ? env->launches : -1; }
+
+int fxenv_set_reset_starts(FxEnv* env, const int64_t* lo_host, const int64_t* hi_host, uint64_t seed) {
+  if (!env) return FXENV_E_INVALID;
+  if ((lo_host == nullptr) != (hi_host == nullptr)) return fail(env, FXENV_E_INVALID, "lo_host and hi_host must both be given or both be NULL");
+  int rc = require_ready(env, false);
+  if (rc) return rc;
+  const FxConfig& c = env->P.cfg;
+  const size_t N = (size_t)c.num_envs;
+  std::vector<int64_t> lo(N, 0);
+  std::vector<uint64_t> span(N, 0);
+  if (lo_host) {
+    for (size_t i = 0; i < N; i++) {
+      const int64_t T = env->P.pair[i % c.num_pairs].T;
+      if (!(0 <= lo_host[i] && lo_host[i] <= hi_host[i] && hi_host[i] <= T - 1)) {
+        char buf[160];
+        snprintf(buf, sizeof buf, "start range of env %zu is [%lld, %lld]; it must satisfy 0 <= lo <= hi <= %lld", i,
+                 (long long)lo_host[i], (long long)hi_host[i], (long long)(T - 1));
+        return fail(env, FXENV_E_INVALID, buf);
+      }
+      lo[i] = lo_host[i];
+      span[i] = (uint64_t)(hi_host[i] - lo_host[i]) + 1u;
+    }
+  } else {
+    seed = 0;  // cleared: the state is what it was before any range was set
+  }
+  DeviceGuard g(env->device);
+  FX_CUDA(env, cudaDeviceSynchronize());
+  const FxDeviceState& st = env->P.st;
+  FX_CUDA(env, cudaMemcpy(st.ep_lo, lo.data(), N * 8, cudaMemcpyHostToDevice));
+  FX_CUDA(env, cudaMemcpy(st.ep_span, span.data(), N * 8, cudaMemcpyHostToDevice));
+  FX_CUDA(env, cudaMemcpy(st.ep_seed, &seed, 8, cudaMemcpyHostToDevice));
+  return FXENV_OK;
+}
+
+int fxenv_get_episode_info(FxEnv* env, FxEpisodePtrs* out) {
+  if (!env || !out) return FXENV_E_INVALID;
+  const FxDeviceState& st = env->P.st;
+  out->start = st.start; out->episodes_done = st.ep_done; out->last_episode = st.ep_last;
+  return FXENV_OK;
+}
 
 /* debug (FXENV_TIMELINE=K, timing build): copies the [K][num_envs][2] ticket start / end stamps; returns K or <0 */
 int fxenv_debug_timeline(FxEnv* env, long long* out_host) {

@@ -156,6 +156,13 @@ __device__ __forceinline__ int32_t fx_total_bars(const FxConfig& c, int64_t T, i
   return (int32_t)tb;
 }
 
+__device__ __forceinline__ uint64_t fx_splitmix64(uint64_t z) {
+  z += 0x9E3779B97F4A7C15ull;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
 // LEAN (compile time, see fx_config_is_lean): the BASELINE family of configurations -- discrete actions, no commission /
 // leverage / slippage, backtrader's next-bar child activation, feature_window preprocessor over the 5 OHLCV columns with
 // a rolling z-score, clipping, price window and agent state, finite data.  The specialised kernels leave out every branch
@@ -163,6 +170,63 @@ __device__ __forceinline__ int32_t fx_total_bars(const FxConfig& c, int64_t T, i
 template <bool LEAN = false>
 __device__ __forceinline__ bool fx_uses_running_stats(const FxConfig& c) {
   return LEAN || (c.preproc == FX_PREPROC_FEATURE_WINDOW && c.scaling != FX_SCALING_NONE);
+}
+
+// GymFxEnv.reset of one env, by one thread (fx_reset_kernel; lane 0 of fx_step_env's auto-reset branch).  The episode it
+// ends, if that ever took a step, is latched from the state arrays into ep_last.  The new one starts at `start` (clamped
+// to the table), or, with `draw` and a start range set, at a bar drawn from the range (include/fxenv.h,
+// fxenv_set_reset_starts).  Scalar and out of line: the step kernels' registers belong to the stepping path.
+__device__ __noinline__ void fx_reset_env(const FxKernelParams& P, const int env, int64_t start, const bool draw) {
+  const FxConfig& c = P.cfg;
+  const FxDeviceState& st = P.st;
+  const FxPairTable& tb = P.pair[env % c.num_pairs];
+  const int32_t k = st.ep_begun[env];
+  const uint32_t flags = st.flags[env];
+  if (flags & FX_FLAG_STARTED) {
+    double* r = st.ep_last + (int64_t)env * FXENV_EPISODE_STATS;
+    const double* rs = st.rstats + (int64_t)env * FX_RS_N;
+    r[FXENV_EP_START] = (double)st.start[env];
+    r[FXENV_EP_BARS] = (double)st.bar_index[env];
+    r[FXENV_EP_EQUITY] = st.equity[env];
+    r[FXENV_EP_COMMISSION] = st.commission_paid[env];
+    r[FXENV_EP_END_FLAGS] = (double)(flags & (FX_FLAG_TERMINATED | FX_FLAG_EXHAUSTED | FX_FLAG_BROKE));
+    r[FXENV_EP_DD_MAX_PCT] = rs[FX_RS_DD_MAX_PCT];
+    r[FXENV_EP_DD_MAX_MONEY] = rs[FX_RS_DD_MAX_MONEY];
+    r[FXENV_EP_PNL_NET] = rs[FX_RS_PNL_NET];
+    r[FXENV_EP_PNL_SQ] = rs[FX_RS_PNL_SQ];
+    r[FXENV_EP_OPENED] = rs[FX_RS_OPENED];
+    r[FXENV_EP_CLOSED] = (double)st.trades[env];
+    r[FXENV_EP_WON] = rs[FX_RS_WON];
+    r[FXENV_EP_LOST] = rs[FX_RS_LOST];
+    r[FXENV_EP_INDEX] = (double)(k - 1);
+    st.ep_done[env] += 1;
+  }
+  st.ep_begun[env] = k + 1;
+  const uint64_t span = st.ep_span[env];
+  if (draw && span != 0) {
+    const uint64_t h = fx_splitmix64(st.ep_seed[0] ^ (((uint64_t)(uint32_t)env << 32) | (uint64_t)(uint32_t)k));
+    start = st.ep_lo[env] + (int64_t)__umul64hi(h, span);
+  }
+  if (start < 0) start = 0;
+  if (start > tb.T - 1) start = tb.T - 1;
+  FxEnvRegs e;
+  fx_reset_regs(c, e, tb.candles[start * (int64_t)c.n_cols + 3]);
+  fx_store_all(st, env, e);
+  st.start[env] = start;
+  st.t[env] = 0;
+  st.total_bars[env] = fx_total_bars(c, tb.T, start);
+  st.n_orders[env] = 0;
+  st.n_acc[env] = 0;
+  st.sub_need[env] = 0.0;
+  for (int j = 0; j < FX_RS_N; j++) st.rstats[(int64_t)env * FX_RS_N + j] = (j == FX_RS_DD_MAXVALUE) ? c.initial_cash : 0.0;
+  for (int j = 0; j < 5; j++) st.nbar[(int64_t)env * 6 + j] = tb.candles[start * (int64_t)c.n_cols + (j < 4 ? j : c.price_col)];
+  if (fx_uses_running_stats(c)) {
+    for (int f = 0; f < c.n_features; f++) {
+      const int64_t wi = ((int64_t)env * FXENV_MAX_FEATURES + f) * 2;
+      st.welford[wi] = tb.candles[start * (int64_t)c.n_cols + c.feature_cols[f]];
+      st.welford[wi + 1] = 0.0;
+    }
+  }
 }
 
 // z-score statistics of the history window ending at local row s-1, for lane f < F: {mean, 1/std}.
@@ -703,19 +767,13 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   //      with auto_reset (build-side extension) the env restarts its episode window instead
   if (flags & FX_FLAG_TERMINATED) {
     if (c.auto_reset) {
+      // a new episode (fx_reset_env, lane 0: the finished one is latched, the start drawn, the state arrays re-initialised);
+      // the warp then continues from the new start
+      if (lane == 0) fx_reset_env(P, env, start, true);
+      __syncwarp();
+      start = st.start[env];
       total_bars = fx_total_bars(c, tb.T, start);
       fx_reset_regs(c, e, tb.candles[start * (int64_t)C + 3]);
-      if (fx_uses_running_stats<LEAN>(c) && lane < c.n_features) {
-        const int64_t wi = ((int64_t)env * FXENV_MAX_FEATURES + lane) * 2;
-        st.welford[wi] = tb.candles[start * (int64_t)C + c.feature_cols[lane]];
-        st.welford[wi + 1] = 0.0;
-      }
-      if (lane < 5) st.nbar[(int64_t)env * 6 + lane] = tb.candles[start * (int64_t)C + (lane < 4 ? lane : c.price_col)];
-      if (lane < FX_RS_N) st.rstats[(int64_t)env * FX_RS_N + lane] = (lane == FX_RS_DD_MAXVALUE) ? c.initial_cash : 0.0;
-      if (lane == 0) {
-        fx_store_all(st, env, e);
-        st.t[env] = 0; st.total_bars[env] = total_bars; st.n_orders[env] = 0; st.n_acc[env] = 0; st.sub_need[env] = 0.0;
-      }
     } else {
       e.flags = flags;
       e.bar_index = t + 1;
@@ -1223,28 +1281,7 @@ __global__ void fx_reset_kernel(const __grid_constant__ FxKernelParams P, const 
     st.dd_peak[env] = 0.0;
   }
   if (mask && !mask[env]) return;
-  const FxPairTable& tb = P.pair[env % c.num_pairs];
-  int64_t start = start_bar ? start_bar[env] : st.start[env];
-  if (start < 0) start = 0;
-  if (start > tb.T - 1) start = tb.T - 1;
-  FxEnvRegs e;
-  fx_reset_regs(c, e, tb.candles[start * (int64_t)c.n_cols + 3]);
-  fx_store_all(st, env, e);
-  st.start[env] = start;
-  st.t[env] = 0;
-  st.total_bars[env] = fx_total_bars(c, tb.T, start);
-  st.n_orders[env] = 0;
-  st.n_acc[env] = 0;
-  st.sub_need[env] = 0.0;
-  for (int j = 0; j < FX_RS_N; j++) st.rstats[(int64_t)env * FX_RS_N + j] = (j == FX_RS_DD_MAXVALUE) ? c.initial_cash : 0.0;
-  for (int j = 0; j < 5; j++) st.nbar[(int64_t)env * 6 + j] = tb.candles[start * (int64_t)c.n_cols + (j < 4 ? j : c.price_col)];
-  if (fx_uses_running_stats(c)) {
-    for (int f = 0; f < c.n_features; f++) {
-      const int64_t wi = ((int64_t)env * FXENV_MAX_FEATURES + f) * 2;
-      st.welford[wi] = tb.candles[start * (int64_t)c.n_cols + c.feature_cols[f]];
-      st.welford[wi + 1] = 0.0;
-    }
-  }
+  fx_reset_env(P, env, start_bar ? start_bar[env] : st.start[env], start_bar == nullptr);
 }
 
 // writes the observation of the current state (what reset() returns): one warp per env

@@ -37,6 +37,14 @@ struct FxDeviceState {
   double* welford;   // [N][FXENV_MAX_FEATURES][2] running {mean, M2} of each feature column over rows [0, s)
   uint32_t* o_meta;  // [N][cap + FXO_SLACK]  order table, entry-major per env (a warp scans one env coalesced)
   double *o_p0, *o_p1, *o_sz;
+  // episode starts / records (fxenv_set_reset_starts, fxenv_get_episode_info; fx_episode_begin): in the slab rather
+  // than in FxKernelParams, so that snapshots carry them and the cached graphs (P captured by value) stay valid
+  int64_t* ep_lo;      // [N] first start bar of the range
+  uint64_t* ep_span;   // [N] hi - lo + 1; 0 = no range: an episode restarts at its current start
+  uint64_t* ep_seed;   // [1]
+  int32_t* ep_begun;   // [N] episodes begun since create (the k of the next draw)
+  int32_t* ep_done;    // [N] episodes recorded
+  double* ep_last;     // [N][FXENV_EPISODE_STATS] record of the last finished episode
 };
 
 #define FX_NSTAMP 12

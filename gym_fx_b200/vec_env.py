@@ -285,6 +285,80 @@ class VecFxEnv:
         return {"trades": trades, "sqn": {"sqn": sqn, "trades": closed}, "sharpe": {}, "time_return": {},
                 "drawdown": {"max": {"drawdown": float(rs[R["dd_max_pct"]]), "moneydown": float(rs[R["dd_max_money"]])}}}
 
+    # ------------------------------------------------------------------ episode starts / records
+    def set_episode_starts(self, lo, hi=None, seed: int = 0):
+        """Draw the start bar of every new episode -- each auto-reset, and reset() without start_bars -- uniformly from the
+        inclusive range [lo_i, hi_i] of rows of env i's table, by a counter-based rule of (seed, env, episode number):
+        reproducible, and the same in snapshots (include/fxenv.h fxenv_set_reset_starts).  lo / hi: ints (every env) or
+        int [N] arrays; with several pairs of different lengths use arrays.  set_episode_starts(None) clears the ranges:
+        an episode then restarts at its current start, as without them."""
+        N = self.num_envs
+        if lo is None:
+            if hi is not None:
+                raise ValueError("hi must be None when lo is None")
+            lo_a = hi_a = None
+        else:
+            if hi is None:
+                raise ValueError("hi is required with lo")
+            lo_a, hi_a = (np.ascontiguousarray(np.broadcast_to(np.asarray(v), (N,)), dtype=np.int64) if np.ndim(v) == 0
+                          else np.ascontiguousarray(np.asarray(v), dtype=np.int64) for v in (lo, hi))
+            for name, v, a in (("lo", lo, lo_a), ("hi", hi, hi_a)):
+                if a.shape != (N,):
+                    raise ValueError(f"{name} must be a scalar or have {N} elements, got shape {np.shape(v)}")
+                if not np.array_equal(a, np.broadcast_to(np.asarray(v), (N,))):
+                    raise ValueError(f"{name} must hold integers")
+            T = np.asarray([self.total_rows[i % len(self.total_rows)] for i in range(N)], np.int64)
+            bad = np.nonzero((lo_a < 0) | (lo_a > hi_a) | (hi_a > T - 1))[0]
+            if bad.size:
+                i = int(bad[0])
+                raise ValueError(f"start range of env {i} is [{lo_a[i]}, {hi_a[i]}]; it must satisfy 0 <= lo <= hi <= "
+                                 f"{T[i] - 1} (rows of its table - 1)")
+        seed = int(seed)
+        if not 0 <= seed < 2**64:
+            raise ValueError("seed must be in [0, 2**64)")
+        with torch.cuda.device(self.device):
+            rc = self.L.fxenv_set_reset_starts(self._h, None if lo_a is None else lo_a.ctypes.data,
+                                               None if hi_a is None else hi_a.ctypes.data, seed)
+        if rc == -1:
+            raise ValueError(self.L.fxenv_last_error(self._h).decode())
+        _native.check(self.L, self._h, rc, "fxenv_set_reset_starts")
+
+    def _episode_views(self):
+        v = self._info_views.get("episodes")
+        if v is None:
+            p = _native.FxEpisodePtrs()
+            _native.check(self.L, self._h, self.L.fxenv_get_episode_info(self._h, C.byref(p)), "fxenv_get_episode_info")
+            N, E = self.num_envs, _native.EPISODE_STATS
+            v = (_tensor_from_ptr(p.start, N, torch.int64, self.device), _tensor_from_ptr(p.episodes_done, N, torch.int32, self.device),
+                 _tensor_from_ptr(p.last_episode, N * E, torch.float64, self.device).view(N, E))
+            self._info_views["episodes"] = v
+        return v
+
+    def episode_stats(self) -> Dict[str, Any]:
+        """The record of each env's last finished episode (latched when a reset -- auto or explicit -- ended it), as device
+        tensors: what RecordEpisodeStatistics / GymFxEnv.summary() would report for it.  `episodes_done` counts the
+        records (0: nothing recorded yet, the fields are then 0); `start` is the first bar of the CURRENT episode,
+        `episode_start` that of the recorded one.  end_flags: FX_FLAG_TERMINATED | EXHAUSTED | BROKE bits, 0 = cut short
+        by a reset.  total_return, avg_trade_pnl (NaN without closed trades) and sqn are derived as in summary()."""
+        start, done, last = self._episode_views()
+        E = _native.EP
+        col = {k: last[:, j] for k, j in E.items()}
+        ic = float(self.cfg.initial_cash)
+        closed = col["closed"]
+        nan = torch.full_like(closed, float("nan"))
+        return {
+            "start": start, "episodes_done": done, "episode_start": col["start"].to(torch.int64),
+            "bars": col["bars"].to(torch.int32), "final_equity": col["equity"],
+            "total_return": col["equity"] / ic - 1.0 if ic else torch.zeros_like(col["equity"]),
+            "commission_paid": col["commission"], "end_flags": col["end_flags"].to(torch.int32),
+            "max_drawdown_pct": col["dd_max_pct"], "max_drawdown_money": col["dd_max_money"],
+            "pnl_net": col["pnl_net"], "pnl_sq": col["pnl_sq"],
+            "trades_total": col["opened"].to(torch.int64), "trades_closed": closed.to(torch.int64),
+            "trades_won": col["won"].to(torch.int64), "trades_lost": col["lost"].to(torch.int64),
+            "avg_trade_pnl": torch.where(closed > 0, col["pnl_net"] / closed.clamp(min=1.0), nan),
+            "sqn": self._sqn(col["pnl_net"], col["pnl_sq"], closed), "episode_index": col["index"].to(torch.int64),
+        }
+
     # ------------------------------------------------------------------ closed loop (policy on the device)
     def make_policy(self, weights=None) -> "FusedPolicy":
         """An actor-critic MLP(obs_dim, 256, 256) evaluated by the fused tensor-core kernel (fxenv.h: FxPolicy)."""

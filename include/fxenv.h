@@ -237,6 +237,49 @@ int fxenv_set_state(FxEnv* env, const void* buf_host, int64_t nbytes);
 /* Kernels launched by this handle since creation (bench.py's gpu_launches). */
 int64_t fxenv_launch_count(const FxEnv* env);
 
+/* ---- episode starts and episode records (no reference counterpart: a Gymnasium vector env begins a NEW episode on
+ * auto-reset, and RecordEpisodeStatistics keeps the results of the one that ended) ----------------------------------
+ * Start ranges: env i may be given an inclusive range [lo_i, hi_i] of start bars (rows of its pair's table) and the
+ * handle a 64-bit seed.  An episode begun from the ranges -- every auto-reset, and fxenv_reset with start_bar_dev == NULL
+ * (an explicit start_bar_dev still wins) -- starts at
+ *   start = lo + umulhi64(splitmix64(seed ^ ((uint64)i << 32 | (uint32)k)), hi - lo + 1)
+ * where k counts the episodes env i has begun since fxenv_create (explicit resets included) and splitmix64 is the
+ * standard finaliser (z += 0x9E3779B97F4A7C15; z = (z ^ z >> 30) * 0xBF58476D1CE4E5B9; z = (z ^ z >> 27) *
+ * 0x94D049BB133111EB; z ^ z >> 31).  Without ranges (the default) an episode restarts at the env's current start.
+ * lo_host / hi_host: int64 [num_envs], 0 <= lo <= hi <= T_pair - 1 for pair i % num_pairs; both NULL clears the ranges.
+ * Needs the candles loaded (FXENV_E_STATE otherwise).  Synchronous.  The ranges, the seed and the counters live in the
+ * env state: snapshots carry them. */
+int fxenv_set_reset_starts(FxEnv* env, const int64_t* lo_host, const int64_t* hi_host, uint64_t seed);
+
+/* Episode record: when a reset (auto or explicit) ends an episode that has FX_FLAG_STARTED, the env stores what its
+ * analyzers held at the end of it in last_episode and increments episodes_done, once per episode.  The record keeps the
+ * last finished episode per env; the first reset after create records nothing. */
+#define FXENV_EPISODE_STATS 14
+enum {
+  FXENV_EP_START = 0,       /* first bar (table row) of the episode */
+  FXENV_EP_BARS,            /* bars it ran (bridge.bar_index) */
+  FXENV_EP_EQUITY,          /* final equity */
+  FXENV_EP_COMMISSION,      /* commission paid */
+  FXENV_EP_END_FLAGS,       /* flags & (FX_FLAG_TERMINATED | FX_FLAG_EXHAUSTED | FX_FLAG_BROKE); 0 = cut short by a reset */
+  FXENV_EP_DD_MAX_PCT,      /* drawdown.max.drawdown (percent) */
+  FXENV_EP_DD_MAX_MONEY,    /* drawdown.max.moneydown */
+  FXENV_EP_PNL_NET,         /* trades.pnl.net.total */
+  FXENV_EP_PNL_SQ,          /* sum of squares of the closed trades' net pnl */
+  FXENV_EP_OPENED,          /* trades opened */
+  FXENV_EP_CLOSED,          /* trades closed */
+  FXENV_EP_WON, FXENV_EP_LOST,
+  FXENV_EP_INDEX            /* the episode's k (see fxenv_set_reset_starts) */
+};
+
+/* Device pointers into the env state, valid until fxenv_destroy. */
+typedef struct FxEpisodePtrs {
+  const int64_t* start;           /* [num_envs] first bar of the current episode */
+  const int32_t* episodes_done;   /* [num_envs] episodes recorded since create */
+  const double* last_episode;     /* [num_envs][FXENV_EPISODE_STATS], FXENV_EP_* order (zeros until the first record) */
+} FxEpisodePtrs;
+
+int fxenv_get_episode_info(FxEnv* env, FxEpisodePtrs* out);
+
 /* ---- closed loop: a policy on the device between the steps ------------------------------------------------------
  * Replaces the caller loop of app/main.py:57-65 (`action = strategy.decide_action(obs, info, step); env.step(action)`)
  * for a learned actor-critic (BASELINE configs[3]: PPO MLP(256,256)): observation rows never leave the GPU, and the
