@@ -407,7 +407,7 @@ int fxenv_step_many(FxEnv* env, int n_steps, const void* actions_dev, float* obs
                                    tracked ? env->seq_base : 0u, tracked ? env->ticket_base : 0u, !tracked, stream));
     if (tracked) {
       env->seq_base += (unsigned)n_steps;
-      env->ticket_base += (unsigned)(N * (size_t)plan.n_rounds) + (unsigned)(fx_rollout_blocks(env->P) * FX_WARPS);
+      env->ticket_base += (unsigned)(N * (size_t)plan.n_rounds) + (unsigned)fx_rollout_warps(env->P);
     }
     env->launches += 1;
     return FXENV_OK;
@@ -618,6 +618,20 @@ int fxenv_debug_rollout_plan(int num_envs, int resident_warps, int n_steps, int*
   for (; r < pl.n_uniform; r++) starts[r] = r * pl.chunk;
   for (int t = 0; r <= pl.n_rounds; r++, t++) starts[r] = pl.tail_start[t];
   return pl.n_rounds;
+}
+
+/* debug / tests (pure host arithmetic, no CUDA call): whether fxenv_step_many keeps each ticket's order table in shared
+ * memory for a configuration of this window / column count / Sharpe ring (0 unless sharpe_reward) / order capacity;
+ * force = FXENV_ORDER_SMEM (0 or 1) or -1.  Returns 1 (resident) or 0 (global). */
+int fxenv_debug_order_smem(int window_size, int n_cols, int ring_len, int order_capacity, int force) {
+  if (window_size < 1 || n_cols < 1 || ring_len < 0 || order_capacity < 1) return FXENV_E_INVALID;
+  FxKernelParams P = {};
+  P.cfg.window_size = window_size;
+  P.cfg.n_cols = n_cols;
+  P.cfg.reward = ring_len > 0 ? FX_REWARD_SHARPE : FX_REWARD_PNL;
+  P.cfg.sharpe_window = ring_len;
+  P.cap = (order_capacity + 31) & ~31;
+  return fx_order_smem_choice(P, force);
 }
 
 /* debug (FXENV_TIMING=1): copies the [num_envs][FX_NSTAMP] phase stamps of the last step; returns FX_NSTAMP or <0 */

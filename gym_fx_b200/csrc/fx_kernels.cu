@@ -48,9 +48,12 @@ constexpr int kLongUnroll = FX_LONG_UNROLL;  // (a macro is not expanded inside 
 namespace {
 
 // per-warp shared memory: the TMA-staged candle window + z-score statistics (+ the Sharpe ring) + one mbarrier
+// (+ the env's order table in the resident-table rollout kernel)
 struct WarpSmem {
   double *win, *stat, *ring;  // stat: [F][2] = {mean, 1/std} per feature (the layout of the per-bar statistics table)
   double* carry;              // FX_CARRY_*: the env's scalar state between two steps run by the same warp (fx_rollout_kernel)
+  double *op0, *op1, *osz;    // [cap + FXO_SLACK] each: the order table of the env a ticket owns (RESIDENT), else unused
+  uint32_t* ometa;
   unsigned long long* bar;
 };
 
@@ -65,27 +68,49 @@ enum {
   FX_CARRY_NACC_TRADES,                // int2 {n_acc, trades}
   FX_CARRY_START,                      // int64
   FX_CARRY_SHARPE,                     // int2 {deque length, head}; the deque itself stays in WarpSmem::ring
-  FX_CARRY_SHARPE_LAST,                // int32 last step seen by the Sharpe plugin
+  FX_CARRY_SHARPE_LAST,                // int2 {last step seen by the Sharpe plugin, table bound (fx_carry_tab_hi)}
   FX_CARRY_RSTATS,                     // FX_RS_N slots
   FX_CARRY_N = FX_CARRY_RSTATS + FX_RS_N
 };
 
+// RESIDENT: entries [0, hi) of the warp's copy of the order table may differ from global memory (the second int32 of an
+// existing slot: the layout of the other kernels stays as it is)
+__device__ __forceinline__ int32_t* fx_carry_tab_hi(double* carry) {
+  return reinterpret_cast<int32_t*>(carry + FX_CARRY_SHARPE_LAST) + 1;
+}
+
 __host__ __device__ inline int fx_window_doubles(int W, int C) { return (W * C + 2 + 1) & ~1; }  // +1 alignment, even
 
-__host__ __device__ inline size_t fx_warp_smem_bytes(int win_doubles, int ring_len) {
-  size_t b = (size_t)win_doubles * 8 + 2 * FXENV_MAX_FEATURES * 8 + (size_t)ring_len * 8 + FX_CARRY_N * 8 + 16;
+// tab_entries: cap + FXO_SLACK for the resident-table rollout kernel, else 0 (a multiple of 32: 28 B per entry keep the
+// mbarrier 8-byte aligned)
+__host__ __device__ inline size_t fx_warp_smem_bytes(int win_doubles, int ring_len, int tab_entries = 0) {
+  size_t b = (size_t)win_doubles * 8 + 2 * FXENV_MAX_FEATURES * 8 + (size_t)ring_len * 8 + FX_CARRY_N * 8 +
+             (size_t)tab_entries * (3 * 8 + 4) + 16;
   return (b + 15) & ~(size_t)15;
 }
 
-__device__ __forceinline__ WarpSmem fx_carve(unsigned char* base, int win_doubles, int ring_len) {
+__device__ __forceinline__ WarpSmem fx_carve(unsigned char* base, int win_doubles, int ring_len, int tab_entries = 0) {
   WarpSmem w;
   double* d = reinterpret_cast<double*>(base);
   w.win = d; d += win_doubles;
   w.stat = d; d += 2 * FXENV_MAX_FEATURES;
   w.ring = d; d += ring_len;
   w.carry = d; d += FX_CARRY_N;
-  w.bar = reinterpret_cast<unsigned long long*>(d);
+  w.op0 = d; d += tab_entries;
+  w.op1 = d; d += tab_entries;
+  w.osz = d; d += tab_entries;
+  w.ometa = reinterpret_cast<uint32_t*>(d);
+  w.bar = reinterpret_cast<unsigned long long*>(w.ometa + tab_entries);
   return w;
+}
+
+// entries [0, n) of an order table from one copy to the other (global <-> the warp's shared memory), coalesced
+__device__ __forceinline__ void fx_table_copy(uint32_t* __restrict__ dm, double* __restrict__ d0, double* __restrict__ d1,
+                                              double* __restrict__ ds, const uint32_t* __restrict__ sm,
+                                              const double* __restrict__ s0, const double* __restrict__ s1,
+                                              const double* __restrict__ ss, const int n, const int lane) {
+#pragma unroll 4
+  for (int k = lane; k < n; k += 32) { dm[k] = sm[k]; d0[k] = s0[k]; d1[k] = s1[k]; ds[k] = ss[k]; }
 }
 
 // ---- TMA (cp.async.bulk) staging of the env's candle window: rows [left, s) of its episode, one contiguous span ----
@@ -659,7 +684,10 @@ __device__ __forceinline__ uint32_t fx_apply_op(uint32_t m, uint32_t op) {
 // One env-step of one env by one warp (everything between the cross-kernel dependency wait and the release).
 // CARRY (fx_rollout_kernel): the step leaves the env's scalar state in ws.carry and returns true if that record is valid;
 // carry_in = the previous call of this warp was the same env's previous step and returned true.
-template <int STRAT, int REWARD, bool FAST5, bool O16, bool LEAN, bool CARRY = false>
+// RESIDENT (with CARRY): the env's order table lives in ws.op0/op1/osz/ometa while the carry record is valid -- loaded
+// from global memory by a step without carry_in, written back by a step that returns false (terminated branch) and by
+// the caller at the end of its ticket (fx_rollout_kernel).
+template <int STRAT, int REWARD, bool FAST5, bool O16, bool LEAN, bool CARRY = false, bool RESIDENT = false>
 __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void* __restrict__ actions, float* __restrict__ obs,
                                             float* __restrict__ reward, double* __restrict__ reward64,
                                             uint8_t* __restrict__ terminated, const int env, const int lane, const WarpSmem& ws,
@@ -741,13 +769,15 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   if (!LEAN && c.action_mode == FX_ACTION_CONTINUOUS) action_raw_f = reinterpret_cast<const float*>(actions)[FX_OUT_IDX()];
   else action_raw_i = reinterpret_cast<const int32_t*>(actions)[FX_OUT_IDX()];
   // the first 32 orders of the table sit at an address that only depends on the env: they travel with the state
+  // (RESIDENT: the table is read from the warp's shared memory instead, no prefetch)
   const int64_t obase = (int64_t)env * capP;
-  uint32_t* __restrict__ gmeta = st.o_meta + obase;
-  double* __restrict__ gp0 = st.o_p0 + obase;
-  double* __restrict__ gp1 = st.o_p1 + obase;
-  double* __restrict__ gsz = st.o_sz + obase;
-  uint32_t pm0 = gmeta[lane];
-  double pp0 = gp0[lane], pp1 = gp1[lane], psz = gsz[lane];
+  uint32_t* __restrict__ gmeta = RESIDENT ? ws.ometa : st.o_meta + obase;
+  double* __restrict__ gp0 = RESIDENT ? ws.op0 : st.o_p0 + obase;
+  double* __restrict__ gp1 = RESIDENT ? ws.op1 : st.o_p1 + obase;
+  double* __restrict__ gsz = RESIDENT ? ws.osz : st.o_sz + obase;
+  uint32_t pm0 = 0u;
+  double pp0 = 0.0, pp1 = 0.0, psz = 0.0;
+  if (!RESIDENT) { pm0 = gmeta[lane]; pp0 = gp0[lane]; pp1 = gp1[lane]; psz = gsz[lane]; }
 #ifndef FX_NO_RUN_STATS
   const FxRunStatsWarp rs{rsv, lane};
 #else   // A/B timing builds only
@@ -766,6 +796,9 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   // ---- terminated envs: the reference answers (obs, 0.0, True) without touching plugins (app/env.py:137-138);
   //      with auto_reset (build-side extension) the env restarts its episode window instead
   if (flags & FX_FLAG_TERMINATED) {
+    if (RESIDENT && carry_in)  // this step returns false: the next one reloads the table from global memory
+      fx_table_copy(st.o_meta + obase, st.o_p0 + obase, st.o_p1 + obase, st.o_sz + obase, gmeta, gp0, gp1, gsz,
+                    *fx_carry_tab_hi(ws.carry), lane);
     if (c.auto_reset) {
       // a new episode (fx_reset_env, lane 0: the finished one is latched, the start drawn, the state arrays re-initialised);
       // the warp then continues from the new start
@@ -805,11 +838,16 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   else if (t + 1 >= total_bars) exhausted = true;  // strategy.stop(): bridge state unchanged (app/bt_bridge.py:152-155)
   else { t += 1; advance = true; }
   e.flags = flags;
+  const int dbg = LEAN ? 0 : P.debug;
+  if (RESIDENT && !carry_in && !(dbg & 2)) {  // first step of a ticket: the table into shared memory
+    fx_table_copy(gmeta, gp0, gp1, gsz, st.o_meta + obase, st.o_p0 + obase, st.o_p1 + obase, st.o_sz + obase, n, lane);
+    if (lane == 0) *fx_carry_tab_hi(ws.carry) = n;
+    __syncwarp();
+  }
 
   // ---- the broker can start right away (candle + first 32 orders arrived with the state); what only the observation
   //      needs -- the candle window and the bar's z-score statistics -- is fetched by TMA bulk copies into shared
   //      memory while the broker runs, without occupying registers
-  const int dbg = LEAN ? 0 : P.debug;
   const int s_obs = t + 1;  // bar_index after this step
   const double* __restrict__ row = tb.candles + (start + t) * (int64_t)C;
   FxBar b;
@@ -866,7 +904,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       if (n > 0) {
         // ---- check_submitted: the entries created by the previous strategy call are [n_acc, n); their cash bound
         //      was stored when they were created.  If cash covers it nobody can be rejected; otherwise the exact
-        //      sequential simulation (cold path) runs on the table in global memory.
+        //      sequential simulation (cold path) runs on the table in place.
         int first_sub = n_acc;
         bool reload0 = false;
         if (n_acc < n && !(e.cash >= sub_need * 1.001)) {
@@ -887,15 +925,16 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
         int n_fills = 0;
 #endif
         uint32_t carry = 0u;  // operation for the first entry of the next chunk (bracket pair of a parent in lane 31)
-        if (reload0 && lane < n) { pm0 = gmeta[lane]; pp0 = gp0[lane]; pp1 = gp1[lane]; psz = gsz[lane]; }
+        if (!RESIDENT && reload0 && lane < n) { pm0 = gmeta[lane]; pp0 = gp0[lane]; pp1 = gp1[lane]; psz = gsz[lane]; }
         for (int k0 = 0; k0 < n; k0 += 32) {
           const int k = k0 + lane;
           const bool valid = k < n;
           // the chunk in flight: entries [k0+32, k0+64) are requested now and consumed by the next iteration (this
-          // iteration only writes at indices <= k, so what it fetches stays valid)
+          // iteration only writes at indices <= k, so what it fetches stays valid); RESIDENT: read from shared memory
+          if (RESIDENT && valid) { pm0 = gmeta[k]; pp0 = gp0[k]; pp1 = gp1[k]; psz = gsz[k]; }
           const uint32_t m0 = pm0;
           const double p0 = pp0, p1 = pp1, sz = psz;
-          if (k + 32 < n) { pm0 = gmeta[k + 32]; pp0 = gp0[k + 32]; pp1 = gp1[k + 32]; psz = gsz[k + 32]; }
+          if (!RESIDENT && k + 32 < n) { pm0 = gmeta[k + 32]; pp0 = gp0[k + 32]; pp1 = gp1[k + 32]; psz = gsz[k + 32]; }
           uint32_t m = 0u;
           if (valid) {
             m = fx_entry_begin_bar(m0);
@@ -1008,7 +1047,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       }
       const bool has_min = (tb.minutes != nullptr);
       const int64_t minutes = (STRAT == FX_STRATEGY_ATR_SLTP && c.session_filter && has_min) ? tb.minutes[start + t] : 0;
-      // new orders are appended straight to the (compacted) table in global memory; their check_submitted cash
+      // new orders are appended straight to the (compacted) table (RESIDENT: the shared copy); their check_submitted cash
       // bound is accumulated by fx_push and kept in the env state for the next step
       FxOrderTab tg;
       tg.meta = gmeta; tg.p0 = gp0; tg.p1 = gp1; tg.sz = gsz;
@@ -1092,6 +1131,11 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
         *reinterpret_cast<int2*>(cr + FX_CARRY_BARS_N) = make_int2(total_bars, n_final);
         *reinterpret_cast<int2*>(cr + FX_CARRY_NACC_TRADES) = make_int2(n_acc_new, e.trades);
         *reinterpret_cast<long long*>(cr + FX_CARRY_START) = start;
+        if (RESIDENT) {  // every index this ticket wrote is below the largest table size it saw: the write-back range,
+                         // which leaves the global arrays exactly as the global-table kernel does (stale entries included)
+          int32_t* hi = fx_carry_tab_hi(cr);
+          if (n_final > *hi) *hi = n_final;
+        }
       }
     }
   } else {  // timing experiment only (FXENV_DEBUG & 2): cursor only
@@ -1207,11 +1251,15 @@ fx_step_kernel(const __grid_constant__ FxKernelParams P, const void* __restrict_
 // (~20 % of a step at chunk = 1): the chunk length amortises it (fx_rollout_plan).  No deadlock: the ticket an env-step
 // waits for is lower than its own, and every ticket handed out belongs to a running warp that needs nothing from higher
 // tickets.  seq[] and the counter are epoch-based (see below), or zeroed by a stream-ordered memset inside captures.
+// RESIDENT (FxKernelParams::order_smem): a ticket keeps its env's order table in the warp's shared memory, loaded by its
+// first step and written back before the release -- no order-table round trip on the steps in between.  The table
+// (28 B per entry) does not fit next to 16 one-warp CTAs per SM with their 1 KB reservation each: FX_RES_WARPS warps per
+// CTA instead, still 16 warps per SM (the warps are independent; there is no block barrier).
 #ifndef FX_ROLLOUT_MIN_BLOCKS
 #define FX_ROLLOUT_MIN_BLOCKS FX_MIN_BLOCKS
 #endif
-template <int STRAT, int REWARD, bool FAST5, bool LEAN>
-__global__ void __launch_bounds__(FX_WARPS * 32, FX_ROLLOUT_MIN_BLOCKS)
+template <int STRAT, int REWARD, bool FAST5, bool LEAN, bool RESIDENT>
+__global__ void __launch_bounds__(FX_ROLLOUT_WARPS(RESIDENT) * 32, FX_ROLLOUT_MIN_BLOCKS * FX_WARPS / FX_ROLLOUT_WARPS(RESIDENT))
 fx_rollout_kernel(const __grid_constant__ FxKernelParams P, const char* __restrict__ actions, float* __restrict__ obs,
                   const int obs_slots, float* __restrict__ reward, uint8_t* __restrict__ terminated,
                   const __grid_constant__ FxChunkPlan plan, const unsigned seq_base, const unsigned ticket_base) {
@@ -1220,7 +1268,8 @@ fx_rollout_kernel(const __grid_constant__ FxKernelParams P, const char* __restri
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int ring_len = (REWARD == FX_REWARD_SHARPE) ? c.sharpe_window : 0;
   const int win_doubles = fx_window_doubles(c.window_size, c.n_cols);
-  const WarpSmem ws = fx_carve(fx_smem + (size_t)warp * fx_warp_smem_bytes(win_doubles, ring_len), win_doubles, ring_len);
+  const int tab = RESIDENT ? P.cap + FXO_SLACK : 0;
+  const WarpSmem ws = fx_carve(fx_smem + (size_t)warp * fx_warp_smem_bytes(win_doubles, ring_len, tab), win_doubles, ring_len, tab);
   asm volatile("griddepcontrol.launch_dependents;");  // the next batch's launch latency hides behind this one
   fx_window_init(lane, ws);
   const unsigned N = (unsigned)c.num_envs;
@@ -1255,8 +1304,8 @@ fx_rollout_kernel(const __grid_constant__ FxKernelParams P, const char* __restri
 #if defined(FXENV_ENABLE_TIMING) || defined(FXENV_ENABLE_TIMELINE)
       if (P.timeline && lane == 0) { long long g__; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g__)); P.timeline[((size_t)k * N + env) * 2] = g__; }
 #endif
-      carry = fx_step_env<STRAT, REWARD, FAST5, false, LEAN, true>(P, actions, obs, reward, nullptr, terminated, (int)env, lane, ws,
-                                                                 phase, k * N, slot_row, nullptr, 0, carry);
+      carry = fx_step_env<STRAT, REWARD, FAST5, false, LEAN, true, RESIDENT>(P, actions, obs, reward, nullptr, terminated, (int)env,
+                                                                           lane, ws, phase, k * N, slot_row, nullptr, 0, carry);
       slot_row += N;
       if (slot_row == (unsigned)obs_slots * N) slot_row = 0u;
       __syncwarp();
@@ -1264,6 +1313,12 @@ fx_rollout_kernel(const __grid_constant__ FxKernelParams P, const char* __restri
 #if defined(FXENV_ENABLE_TIMING) || defined(FXENV_ENABLE_TIMELINE)
       if (P.timeline && lane == 0) { long long g__; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g__)); P.timeline[((size_t)k * N + env) * 2 + 1] = g__; }
 #endif
+    }
+    if (RESIDENT && carry) {  // the shared copy is the current table: back to global memory, published by the release
+      const int64_t ob = (int64_t)env * (P.cap + FXO_SLACK);
+      const int n = *fx_carry_tab_hi(ws.carry);
+      fx_table_copy(P.st.o_meta + ob, P.st.o_p0 + ob, P.st.o_p1 + ob, P.st.o_sz + ob, ws.ometa, ws.op0, ws.op1, ws.osz, n, lane);
+      __syncwarp();
     }
     if (lane == 0) fx_st_release(P.seq + env, (int)(seq_base + k_end));
     g = __shfl_sync(FX_FULL, g_next, 0);
@@ -1342,10 +1397,14 @@ StepKernel pick_step_mode(int mode) {
   if (mode == 2) return fx_step_kernel<STRAT, REWARD, true, true>;
   return mode == 1 ? fx_step_kernel<STRAT, REWARD, true, false> : fx_step_kernel<STRAT, REWARD, false, false>;
 }
+template <int STRAT, int REWARD, bool RESIDENT>
+RolloutKernel pick_rollout_table(int mode) {
+  if (mode == 2) return fx_rollout_kernel<STRAT, REWARD, true, true, RESIDENT>;
+  return mode == 1 ? fx_rollout_kernel<STRAT, REWARD, true, false, RESIDENT> : fx_rollout_kernel<STRAT, REWARD, false, false, RESIDENT>;
+}
 template <int STRAT, int REWARD>
-RolloutKernel pick_rollout_mode(int mode) {
-  if (mode == 2) return fx_rollout_kernel<STRAT, REWARD, true, true>;
-  return mode == 1 ? fx_rollout_kernel<STRAT, REWARD, true, false> : fx_rollout_kernel<STRAT, REWARD, false, false>;
+RolloutKernel pick_rollout_mode(int mode, bool resident) {
+  return resident ? pick_rollout_table<STRAT, REWARD, true>(mode) : pick_rollout_table<STRAT, REWARD, false>(mode);
 }
 template <int STRAT>
 StepKernel pick_reward(int reward, int mode) {
@@ -1356,11 +1415,11 @@ StepKernel pick_reward(int reward, int mode) {
   }
 }
 template <int STRAT>
-RolloutKernel pick_rollout_reward(int reward, int mode) {
+RolloutKernel pick_rollout_reward(int reward, int mode, bool resident) {
   switch (reward) {
-    case FX_REWARD_PNL: return pick_rollout_mode<STRAT, FX_REWARD_PNL>(mode);
-    case FX_REWARD_SHARPE: return pick_rollout_mode<STRAT, FX_REWARD_SHARPE>(mode);
-    default: return pick_rollout_mode<STRAT, FX_REWARD_DD>(mode);
+    case FX_REWARD_PNL: return pick_rollout_mode<STRAT, FX_REWARD_PNL>(mode, resident);
+    case FX_REWARD_SHARPE: return pick_rollout_mode<STRAT, FX_REWARD_SHARPE>(mode, resident);
+    default: return pick_rollout_mode<STRAT, FX_REWARD_DD>(mode, resident);
   }
 }
 
@@ -1377,10 +1436,11 @@ StepKernel pick_kernel(const FxKernelParams& P, int lean = -1) {
 
 RolloutKernel pick_rollout(const FxKernelParams& P, int lean = -1) {
   const int mode = kernel_mode(P, lean < 0 ? P.lean : lean);
+  const bool res = P.order_smem != 0;
   switch (P.cfg.strategy) {
-    case FX_STRATEGY_DEFAULT: return pick_rollout_reward<FX_STRATEGY_DEFAULT>(P.cfg.reward, mode);
-    case FX_STRATEGY_FIXED_SLTP: return pick_rollout_reward<FX_STRATEGY_FIXED_SLTP>(P.cfg.reward, mode);
-    default: return pick_rollout_reward<FX_STRATEGY_ATR_SLTP>(P.cfg.reward, mode);
+    case FX_STRATEGY_DEFAULT: return pick_rollout_reward<FX_STRATEGY_DEFAULT>(P.cfg.reward, mode, res);
+    case FX_STRATEGY_FIXED_SLTP: return pick_rollout_reward<FX_STRATEGY_FIXED_SLTP>(P.cfg.reward, mode, res);
+    default: return pick_rollout_reward<FX_STRATEGY_ATR_SLTP>(P.cfg.reward, mode, res);
   }
 }
 
@@ -1389,21 +1449,52 @@ size_t step_smem_bytes(const FxKernelParams& P) {
   return fx_warp_smem_bytes(fx_window_doubles(P.cfg.window_size, P.cfg.n_cols), ring_len) * FX_WARPS;
 }
 
+int rollout_cta_warps(const FxKernelParams& P) { return FX_ROLLOUT_WARPS(P.order_smem != 0); }
+
+// per CTA of fx_rollout_kernel, for the variant `resident`
+size_t rollout_smem_bytes(const FxKernelParams& P, bool resident) {
+  const int ring_len = (P.cfg.reward == FX_REWARD_SHARPE) ? P.cfg.sharpe_window : 0;
+  const int tab = resident ? P.cap + FXO_SLACK : 0;
+  return fx_warp_smem_bytes(fx_window_doubles(P.cfg.window_size, P.cfg.n_cols), ring_len, tab) * FX_ROLLOUT_WARPS(resident);
+}
+
 size_t observe_smem_bytes(const FxKernelParams& P) {
   return fx_warp_smem_bytes(fx_window_doubles(P.cfg.window_size, P.cfg.n_cols), 0) * FX_WARPS;
 }
 
+// shared-memory carve-out (percent of the SM's 228 KB) that holds `ctas` CTAs of `smem` bytes (+1 KB system use each)
+int carveout_pct(size_t ctas, size_t smem) {
+  const size_t want = ctas * (smem + 1024);
+  int pct = (int)((want * 100 + 228 * 1024 - 1) / (228 * 1024));
+  if (pct > 100) pct = 100;
+  if (const char* cv = getenv("FXENV_CARVEOUT")) { const int v = atoi(cv); if (v >= pct && v <= 100) pct = v; }  // measurements
+  return pct;
+}
+
 }  // namespace
+
+// The resident-table rollout kernel when its CTAs fit an SM as many warps as the global-table one runs (16): each
+// CTA at most 227 KB, and (16 / FX_ROLLOUT_WARPS(true)) CTAs plus their 1 KB reservations at most the SM's 228 KB.
+// force: 0 / 1 = FXENV_ORDER_SMEM (measurements, tests), < 0 = decide by the budget.
+int fx_order_smem_choice(const FxKernelParams& P, int force) {
+  if (force >= 0) return force ? 1 : 0;
+  const size_t cta = rollout_smem_bytes(P, true);
+  const size_t ctas = (size_t)FX_ROLLOUT_MIN_BLOCKS * FX_WARPS / FX_ROLLOUT_WARPS(true);
+  return (cta <= 227 * 1024 && ctas * (cta + 1024) <= 228 * 1024) ? 1 : 0;
+}
 
 // dynamic shared memory above the 48 KB default needs an explicit opt-in per kernel
 cudaError_t fx_configure_kernels(FxKernelParams& P) {
   const size_t smem = step_smem_bytes(P);
   if (smem > 227 * 1024) return cudaErrorInvalidValue;
+  const char* os = getenv("FXENV_ORDER_SMEM");
+  P.order_smem = fx_order_smem_choice(P, os ? atoi(os) : -1);
+  const size_t rsmem = rollout_smem_bytes(P, P.order_smem != 0);
+  if (rsmem > 227 * 1024) return cudaErrorInvalidValue;
   // ask for enough shared-memory carve-out that FX_MIN_BLOCKS CTAs (+1 KB system use each) fit on an SM
-  const size_t want = (size_t)FX_MIN_BLOCKS * (smem + 1024);
-  int pct = (int)((want * 100 + 228 * 1024 - 1) / (228 * 1024));
-  if (pct > 100) pct = 100;
-  if (const char* cv = getenv("FXENV_CARVEOUT")) { const int v = atoi(cv); if (v >= pct && v <= 100) pct = v; }  // measurements
+  const int pct = carveout_pct(FX_MIN_BLOCKS, smem);
+  const int rcta = rollout_cta_warps(P);
+  const int rpct = carveout_pct((size_t)FX_ROLLOUT_MIN_BLOCKS * FX_WARPS / rcta, rsmem);
   int dev = 0, sms = 0;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -1413,17 +1504,19 @@ cudaError_t fx_configure_kernels(FxKernelParams& P) {
   for (int lean = 0; lean <= (P.fast_features == 5 ? 1 : 0); lean++) {
     cudaError_t e = cudaFuncSetAttribute(pick_kernel(P, lean), cudaFuncAttributePreferredSharedMemoryCarveout, pct);
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(pick_rollout(P, lean), cudaFuncAttributePreferredSharedMemoryCarveout, pct);
+    e = cudaFuncSetAttribute(pick_rollout(P, lean), cudaFuncAttributePreferredSharedMemoryCarveout, rpct);
     if (e != cudaSuccess) return e;
     if (smem > 48 * 1024) {
       e = cudaFuncSetAttribute(pick_kernel(P, lean), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return e;
-      e = cudaFuncSetAttribute(pick_rollout(P, lean), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    }
+    if (rsmem > 48 * 1024) {
+      e = cudaFuncSetAttribute(pick_rollout(P, lean), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rsmem);
       if (e != cudaSuccess) return e;
     }
     // how many CTAs of the persistent rollout kernel the device holds at once (= its grid size)
     int per_sm = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pick_rollout(P, lean), FX_WARPS * 32, smem);
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pick_rollout(P, lean), rcta * 32, rsmem);
     if (e != cudaSuccess) return e;
     if (P.resident_blocks == 0 || sms * per_sm < P.resident_blocks) P.resident_blocks = sms * per_sm;
   }
@@ -1463,9 +1556,12 @@ cudaError_t fx_launch_step(const FxKernelParams& P, const void* actions, float* 
 }
 
 int fx_rollout_blocks(const FxKernelParams& P) {
-  int blocks = (P.cfg.num_envs + FX_WARPS - 1) / FX_WARPS;
+  const int w = rollout_cta_warps(P);
+  int blocks = (P.cfg.num_envs + w - 1) / w;
   return blocks > P.resident_blocks ? P.resident_blocks : blocks;
 }
+
+int fx_rollout_warps(const FxKernelParams& P) { return fx_rollout_blocks(P) * rollout_cta_warps(P); }
 
 // The rounds of a batch (FxChunkPlan): every ticket of round r is one env for the steps [start_r, start_{r+1}).  A longer
 // chunk removes hand-overs (fence + sequence word + acquire round trip per ticket) but coarsens the work units: uniform chunks that leave >= 6 tickets per resident warp, at most 64 steps, the remainder as a
@@ -1476,7 +1572,7 @@ int fx_rollout_blocks(const FxKernelParams& P) {
 FxChunkPlan fx_rollout_plan(const FxKernelParams& P, int n_steps) {
   const char* fe = getenv("FXENV_CHUNK");  // read per launch: tests switch it between batches
   const int forced = fe ? atoi(fe) : 0;
-  const long long warps = (long long)fx_rollout_blocks(P) * FX_WARPS;
+  const long long warps = fx_rollout_warps(P);
   const long long N = P.cfg.num_envs;
   int chunk;
   if (forced > 0) chunk = forced;
@@ -1506,8 +1602,8 @@ cudaError_t fx_launch_rollout(const FxKernelParams& P, const void* actions, floa
   }
   cudaLaunchConfig_t lc = {};
   lc.gridDim = dim3(fx_rollout_blocks(P));
-  lc.blockDim = dim3(FX_WARPS * 32);
-  lc.dynamicSmemBytes = step_smem_bytes(P);
+  lc.blockDim = dim3(rollout_cta_warps(P) * 32);
+  lc.dynamicSmemBytes = rollout_smem_bytes(P, P.order_smem != 0);
   lc.stream = stream;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;

@@ -76,6 +76,7 @@ struct FxKernelParams {
   int32_t any_binary;       // 1: some feature column is a binary pass-through (feature_binary[])
   int32_t lean;             // 1: the configuration qualifies for the specialised kernels (fx_config_is_lean)
   int32_t num_sms;          // SMs of the device (fx_rollout_kernel: CTA b is the (b / num_sms)-th CTA of its SM)
+  int32_t order_smem;       // 1: fx_rollout_kernel keeps each ticket's order table in shared memory (fx_order_smem_choice)
 };
 
 // warps (= envs) per CTA of the step kernel.  One warp per CTA lets the second wave back-fill SM slots as soon as a
@@ -90,6 +91,12 @@ struct FxKernelParams {
 #ifndef FX_MIN_BLOCKS
 #define FX_MIN_BLOCKS (16 / FX_WARPS)   // 16 warps per SM => 128 registers
 #endif
+// warps per CTA of fx_rollout_kernel: with the order table resident in shared memory (13.7 KB per warp for W=128 and
+// 256 orders), 4 warps share one 1 KB per-CTA reservation, so that 16 warps still fit an SM's 228 KB
+#ifndef FX_RES_WARPS
+#define FX_RES_WARPS 4
+#endif
+#define FX_ROLLOUT_WARPS(resident) ((resident) ? FX_RES_WARPS : FX_WARPS)
 
 // host-callable launchers (fx_kernels.cu)
 // one step of the envs [env_begin, env_end) (env_end < 0: all); the array arguments are the bases for env 0
@@ -123,4 +130,6 @@ cudaError_t fx_launch_rollout(const FxKernelParams& P, const void* actions, floa
                               uint8_t* terminated, const FxChunkPlan& plan, unsigned seq_base, unsigned ticket_base,
                               bool reset_words, cudaStream_t stream);
 int fx_rollout_blocks(const FxKernelParams& P);
+int fx_rollout_warps(const FxKernelParams& P);  // warps of a fx_rollout_kernel launch (each draws one ticket past the last)
+int fx_order_smem_choice(const FxKernelParams& P, int force);
 FxChunkPlan fx_rollout_plan(const FxKernelParams& P, int n_steps);  // the host's ticket accounting needs n_rounds
