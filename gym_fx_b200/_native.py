@@ -31,6 +31,7 @@ EXPORTS = [
     "fxenv_state_bytes", "fxenv_get_state", "fxenv_set_state", "fxenv_launch_count", "fxenv_step_many_engine",
     "fxenv_policy_create", "fxenv_policy_set_weights", "fxenv_policy_destroy", "fxenv_rollout", "fxenv_policy_sync_timeouts",
     "fxenv_rollout_ex", "fxenv_policy_peek", "fxenv_set_reset_starts", "fxenv_get_episode_info",
+    "fxenv_set_bracket_audit", "fxenv_get_bracket_audit",
 ]
 
 ROLLOUT_GREEDY = 1  # FXENV_ROLLOUT_GREEDY
@@ -58,6 +59,15 @@ class FxEpisodePtrs(C.Structure):
 EPISODE_STATS = 14  # FXENV_EPISODE_STATS
 EP = {"start": 0, "bars": 1, "equity": 2, "commission": 3, "end_flags": 4, "dd_max_pct": 5, "dd_max_money": 6,
       "pnl_net": 7, "pnl_sq": 8, "opened": 9, "closed": 10, "won": 11, "lost": 12, "index": 13}  # FXENV_EP_*
+
+
+class FxAuditPtrs(C.Structure):
+    _fields_ = [("records", C.c_void_p), ("written", C.c_void_p), ("capacity", C.c_int32)]
+
+
+AU_FIELDS = 8  # FXENV_AU_FIELDS
+AU = {"kind": 0, "bar": 1, "episode": 2, "entry": 3, "stop": 4, "limit": 5, "size": 6, "atr": 7}  # FXENV_AU_*
+AU_KIND_LONG, AU_KIND_SHORT, AU_KIND_FORCE_CLOSE = 1, 2, 3  # FXENV_AU_KIND_*
 
 
 INFO_DTYPES = {
@@ -128,6 +138,8 @@ def load():
     L.fxenv_policy_peek.argtypes = [vp, i32, i32, vp, i64, vp]
     L.fxenv_set_reset_starts.argtypes = [vp, vp, vp, C.c_uint64]
     L.fxenv_get_episode_info.argtypes = [vp, C.POINTER(FxEpisodePtrs)]
+    L.fxenv_set_bracket_audit.argtypes = [vp, C.c_int32]
+    L.fxenv_get_bracket_audit.argtypes = [vp, C.POINTER(FxAuditPtrs)]
     if L.fxenv_abi_version() != 2:
         raise FxEnvError("libfxenv.so ABI version mismatch")
     _lib = L

@@ -65,6 +65,8 @@ struct FxEnv {
     uint64_t used = 0;
   } graphs[2];
   uint64_t graph_clock = 0;
+  // bumped whenever P.audit / audit_cap change: a cached rollout graph captured the old P by value (FxPolicy::cached)
+  uint64_t audit_epoch = 0;
 };
 
 namespace {
@@ -265,6 +267,7 @@ int fxenv_destroy(FxEnv* env) {
   cudaFree(env->P.seq);
   cudaFree(env->P.timing);
   cudaFree(env->P.timeline);
+  cudaFree(env->P.audit); cudaFree(env->P.audit_written);
   cudaFree(env->h_actions); cudaFree(env->h_obs); cudaFree(env->h_reward); cudaFree(env->h_term);
   if (env->hstream) cudaStreamDestroy(env->hstream);
   if (env->hcopy) cudaStreamDestroy(env->hcopy);
@@ -594,6 +597,38 @@ int fxenv_get_episode_info(FxEnv* env, FxEpisodePtrs* out) {
   return FXENV_OK;
 }
 
+int fxenv_set_bracket_audit(FxEnv* env, int32_t capacity) {
+  if (!env) return FXENV_E_INVALID;
+  if (capacity < 0) return fail(env, FXENV_E_INVALID, "bracket audit capacity must be >= 0");
+  const uint64_t N = (uint64_t)env->P.cfg.num_envs;
+  const uint64_t records = N * (uint64_t)capacity;
+  if (capacity > 0 && records > (uint64_t)INT64_MAX / (FXENV_AU_FIELDS * sizeof(double)))
+    return fail(env, FXENV_E_INVALID, "bracket audit capacity too large");
+  DeviceGuard g(env->device);
+  FX_CUDA(env, cudaDeviceSynchronize());  // kernels in flight may still write the old ring
+  drop_graph(env);                        // the cached step-many graphs captured the old P
+  env->audit_epoch++;                     // ... and so did each policy's rollout graph (re-captured on its next use)
+  cudaFree(env->P.audit); cudaFree(env->P.audit_written);
+  env->P.audit = nullptr; env->P.audit_written = nullptr; env->P.audit_cap = 0;
+  if (capacity == 0) return FXENV_OK;
+  double* ring = nullptr;
+  int64_t* written = nullptr;
+  cudaError_t e = cudaMalloc(&ring, records * FXENV_AU_FIELDS * sizeof(double));
+  if (e == cudaSuccess) e = cudaMalloc(&written, N * sizeof(int64_t));
+  if (e == cudaSuccess) e = cudaMemset(ring, 0, records * FXENV_AU_FIELDS * sizeof(double));
+  if (e == cudaSuccess) e = cudaMemset(written, 0, N * sizeof(int64_t));
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  if (e != cudaSuccess) { cudaFree(ring); cudaFree(written); return cuda_fail(env, e, "bracket audit ring"); }
+  env->P.audit = ring; env->P.audit_written = written; env->P.audit_cap = capacity;
+  return FXENV_OK;
+}
+
+int fxenv_get_bracket_audit(FxEnv* env, FxAuditPtrs* out) {
+  if (!env || !out) return FXENV_E_INVALID;
+  out->records = env->P.audit; out->written = env->P.audit_written; out->capacity = env->P.audit_cap;
+  return FXENV_OK;
+}
+
 /* debug (FXENV_TIMELINE=K, timing build): copies the [K][num_envs][2] ticket start / end stamps; returns K or <0 */
 int fxenv_debug_timeline(FxEnv* env, long long* out_host) {
   if (!env || !out_host || !env->P.timeline) return FXENV_E_STATE;
@@ -634,6 +669,10 @@ int fxenv_debug_order_smem(int window_size, int n_cols, int ring_len, int order_
   return fx_order_smem_choice(P, force);
 }
 
+/* debug / tests: 1 if the env runs the specialised (LEAN) kernels (fx_config_is_lean, decided once every candle table is
+ * loaded; FXENV_NO_LEAN turns them off), 0 if the general ones, <0 on error. */
+int fxenv_debug_lean(const FxEnv* env) { return env ? env->P.lean : FXENV_E_INVALID; }
+
 /* debug (FXENV_TIMING=1): copies the [num_envs][FX_NSTAMP] phase stamps of the last step; returns FX_NSTAMP or <0 */
 int fxenv_debug_timings(FxEnv* env, long long* out_host) {
   if (!env || !out_host || !env->P.timing) return FXENV_E_STATE;
@@ -667,7 +706,7 @@ struct FxPolicy {
   FxPolicyDev dev;
   bool has_weights = false;
   bool continuous = false;             // FX_ACTION_CONTINUOUS: Gaussian head, float32 actions (fx_policy_kernel<true>)
-  struct { cudaGraphExec_t exec = nullptr; FxRollout io; uint32_t flags = 0; } cached;
+  struct { cudaGraphExec_t exec = nullptr; FxRollout io; uint32_t flags = 0; uint64_t audit_epoch = 0; } cached;
 };
 
 namespace {
@@ -908,8 +947,10 @@ int fxenv_rollout_ex(FxEnv* env, FxPolicy* pol, const FxRollout* io, uint32_t fl
     env->launches += nl;
     return FXENV_OK;
   }
-  // the graph bakes in the buffers, the seed and the flags (greedy or sampling): any change re-captures it
-  if (!pol->cached.exec || memcmp(&pol->cached.io, io, sizeof(FxRollout)) != 0 || pol->cached.flags != flags) {
+  // the graph bakes in the buffers, the seed, the flags (greedy or sampling) and the env's kernel parameters (P, by
+  // value: the bracket audit ring): any change re-captures it
+  if (!pol->cached.exec || memcmp(&pol->cached.io, io, sizeof(FxRollout)) != 0 || pol->cached.flags != flags ||
+      pol->cached.audit_epoch != env->audit_epoch) {
     if (pol->cached.exec) { cudaGraphExecDestroy(pol->cached.exec); pol->cached.exec = nullptr; }
     cudaGraph_t graph = nullptr;
     FX_CUDA(env, cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
@@ -922,6 +963,7 @@ int fxenv_rollout_ex(FxEnv* env, FxPolicy* pol, const FxRollout* io, uint32_t fl
     if (e != cudaSuccess) { pol->cached.exec = nullptr; return cuda_fail(env, e, "cudaGraphInstantiate"); }
     pol->cached.io = *io;
     pol->cached.flags = flags;
+    pol->cached.audit_epoch = env->audit_epoch;
   }
   FX_CUDA(env, cudaGraphLaunch(pol->cached.exec, stream));
   env->launches += nl;

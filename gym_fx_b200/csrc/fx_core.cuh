@@ -523,10 +523,20 @@ FX_HD void fx_session_state(const FxConfig& c, int64_t minutes, bool& in_entry, 
   in_close = !in_entry;
 }
 
+// The decision direct_atr_sltp reports to its bracket audit (strategy_plugins/direct_atr_sltp.py:138-142, :188-191,
+// :199-202): kind FXENV_AU_KIND_* (FXENV_AU_KIND_NONE: no record this call); stop / limit / size / atr as the reference
+// logs them (size = the signed position before the close for a session force-close, whose stop / limit / atr are unset).
+// Set whether or not the orders find room in the table: the reference's order list is unbounded.
+struct FxAudit {
+  int kind;
+  double stop, limit, size, atr;
+};
+
 // ---- BTBridgeStrategy._apply_action at the current bar ------------------------------------------------------------
 // atr / atr_ready: simple-mean ATR of the env's TR deque (only read for FX_STRATEGY_ATR_SLTP).
+// au: the ATR strategy's audit record of this call (the other strategies leave it untouched).
 FX_HD void fx_apply_action(const FxConfig& c, int strategy, FxEnvRegs& e, FxOrderTab& t, int action, const FxBar& b,
-                           int pair, double atr, bool atr_ready, bool has_minutes, int64_t minutes) {
+                           int pair, double atr, bool atr_ready, bool has_minutes, int64_t minutes, FxAudit& au) {
   const double pos = e.psize, pclose = b.c;
   if (strategy == FX_STRATEGY_DEFAULT) {  // app/bt_bridge.py:171-190 (market orders)
     const double size = c.position_size;
@@ -547,10 +557,12 @@ FX_HD void fx_apply_action(const FxConfig& c, int strategy, FxEnvRegs& e, FxOrde
     sl = c.sl_pips * pip;
     tp = c.tp_pips * pip;
   } else {  // direct_atr_sltp.py:110-202
+    au.kind = FXENV_AU_KIND_NONE;
     size = fx_atr_size(c, e.cash, pclose);
     bool in_entry = true, in_close = false;
     if (c.session_filter && has_minutes) fx_session_state(c, minutes, in_entry, in_close);
     if (in_close && pos != 0.0) {
+      au.kind = FXENV_AU_KIND_FORCE_CLOSE; au.size = pos;
       if (fx_room(t, 1, e.flags)) fx_order_close(t, pos, pclose);
       return;
     }
@@ -562,6 +574,13 @@ FX_HD void fx_apply_action(const FxConfig& c, int strategy, FxEnvRegs& e, FxOrde
     if (c.use_min_frac) { const double fl = c.min_sltp_frac * pclose; if (fl > sl) sl = fl; if (fl > tp) tp = fl; }
     if (c.use_max_frac) { const double ce = c.max_sltp_frac * pclose; if (ce < sl) sl = ce; if (ce < tp) tp = ce; }
     if (tp >= pclose) tp = pclose * 0.5;
+    if (action == 1 ? pos <= 0.0 : pos >= 0.0) {
+      const bool buy = action == 1;
+      au.kind = buy ? FXENV_AU_KIND_LONG : FXENV_AU_KIND_SHORT;
+      au.stop = buy ? pclose - sl : pclose + sl;
+      au.limit = buy ? pclose + tp : pclose - tp;
+      au.size = size; au.atr = atr;
+    }
   }
   if (action == 1) {
     if (pos <= 0.0 && fx_room(t, fx_close_need(pos) + 2, e.flags)) {
@@ -574,6 +593,13 @@ FX_HD void fx_apply_action(const FxConfig& c, int strategy, FxEnvRegs& e, FxOrde
       fx_order_bracket(t, false, size, pclose + sl, pclose - tp, pclose);
     }
   }
+}
+
+// The same call for callers that keep no audit.
+FX_HD void fx_apply_action(const FxConfig& c, int strategy, FxEnvRegs& e, FxOrderTab& t, int action, const FxBar& b,
+                           int pair, double atr, bool atr_ready, bool has_minutes, int64_t minutes) {
+  FxAudit au;
+  fx_apply_action(c, strategy, e, t, action, b, pair, atr, atr_ready, has_minutes, minutes, au);
 }
 
 // ---- app/env.py:187-204 ---------------------------------------------------------------------------------------------

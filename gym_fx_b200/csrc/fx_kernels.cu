@@ -681,6 +681,29 @@ __device__ __forceinline__ uint32_t fx_apply_op(uint32_t m, uint32_t op) {
   return m;
 }
 
+// Bracket audit (include/fxenv.h, fxenv_set_bracket_audit): the env's next record into its ring, lane i storing field i
+// (the decision is warp-uniform), then the counter.  One warp owns the env for the step, so no atomics.  Only the
+// FX_KSTRAT_ATR_AUDIT instantiations contain it: the host launches them while the log is on, so the ATR kernels that
+// run with the log off are exactly those of a build without the audit.
+#define FX_KSTRAT_ATR_AUDIT 3  // kernel template STRAT: direct_atr_sltp with the audit store
+__device__ __noinline__ void fx_audit_store(const FxKernelParams& P, const int env, const int lane, const FxAudit& au,
+                                            const int64_t bar, const double entry) {
+  long long w = (lane == 0) ? (long long)P.audit_written[env] : 0ll;
+  w = __shfl_sync(FX_FULL, w, 0);
+  const double nan = __longlong_as_double(0x7FF8000000000000ll);
+  const bool fc = au.kind == FXENV_AU_KIND_FORCE_CLOSE;
+  double v = (double)au.kind;
+  if (lane == FXENV_AU_BAR) v = (double)bar;
+  else if (lane == FXENV_AU_EPISODE) v = (double)(P.st.ep_begun[env] - 1);
+  else if (lane == FXENV_AU_ENTRY) v = entry;
+  else if (lane == FXENV_AU_STOP) v = fc ? nan : au.stop;
+  else if (lane == FXENV_AU_LIMIT) v = fc ? nan : au.limit;
+  else if (lane == FXENV_AU_SIZE) v = au.size;
+  else if (lane == FXENV_AU_ATR) v = fc ? nan : au.atr;
+  if (lane < FXENV_AU_FIELDS) P.audit[((int64_t)env * P.audit_cap + w % P.audit_cap) * FXENV_AU_FIELDS + lane] = v;
+  if (lane == 0) P.audit_written[env] = (int64_t)(w + 1);
+}
+
 // One env-step of one env by one warp (everything between the cross-kernel dependency wait and the release).
 // CARRY (fx_rollout_kernel): the step leaves the env's scalar state in ws.carry and returns true if that record is valid;
 // carry_in = the previous call of this warp was the same env's previous step and returned true.
@@ -700,6 +723,8 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
 #define FX_OBS_ROW() (obs + ((size_t)obs_slot_row + (size_t)env) * (size_t)P.obs_dim)
 #define FX_OUT_IDX() ((size_t)step_row + (size_t)env)
 #define FX_OBS_ROW16() ((O16 && obs16) ? obs16 + (size_t)env * (size_t)stride16 : nullptr)  // bf16 copy (single-step kernel only)
+  constexpr bool ATR = STRAT == FX_STRATEGY_ATR_SLTP || STRAT == FX_KSTRAT_ATR_AUDIT;
+  constexpr int STRATEGY = ATR ? FX_STRATEGY_ATR_SLTP : STRAT;  // what fx_apply_action runs
   const FxConfig& c = P.cfg;
   const FxDeviceState& st = P.st;
   const int C = c.n_cols;
@@ -1022,7 +1047,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
                                                                            : fx_coerce_discrete(action_raw_i);
       double atr = 0.0;
       bool atr_ready = false;
-      if (STRAT == FX_STRATEGY_ATR_SLTP && action != 0) {
+      if (ATR && action != 0) {
         // simple-mean ATR over the env's TR deque; TR(k) is a pure function of the table (SURVEY A.6): lanes fetch the
         // last min(t+1, period) bars in parallel, then the deque-order compensated sum (Python's sum()) runs uniformly
         const int period = c.atr_period;
@@ -1046,13 +1071,16 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
         atr_ready = nb >= period;
       }
       const bool has_min = (tb.minutes != nullptr);
-      const int64_t minutes = (STRAT == FX_STRATEGY_ATR_SLTP && c.session_filter && has_min) ? tb.minutes[start + t] : 0;
+      const int64_t minutes = (ATR && c.session_filter && has_min) ? tb.minutes[start + t] : 0;
       // new orders are appended straight to the (compacted) table (RESIDENT: the shared copy); their check_submitted cash
       // bound is accumulated by fx_push and kept in the env state for the next step
       FxOrderTab tg;
       tg.meta = gmeta; tg.p0 = gp0; tg.p1 = gp1; tg.sz = gsz;
       tg.n = n_live; tg.cap = P.cap; tg.dirty_from = n_live; tg.ndead = 0; tg.sub_need = 0.0; tg.bound_per = LEAN ? 1.0 : fx_bound_per(c);
-      fx_apply_action(c, STRAT, e, tg, action, b, pair, atr, atr_ready, has_min, minutes);
+      FxAudit au;
+      au.kind = FXENV_AU_KIND_NONE;
+      fx_apply_action(c, STRATEGY, e, tg, action, b, pair, atr, atr_ready, has_min, minutes, au);
+      if (STRAT == FX_KSTRAT_ATR_AUDIT && au.kind != FXENV_AU_KIND_NONE) fx_audit_store(P, env, lane, au, start + t, b.c);
       n_final = tg.n;
       sub_need_new = tg.sub_need;
       fx_publish(e, b.c, t);
@@ -1425,22 +1453,27 @@ RolloutKernel pick_rollout_reward(int reward, int mode, bool resident) {
 
 int kernel_mode(const FxKernelParams& P, int lean) { return (lean && P.fast_features == 5) ? 2 : (P.fast_features == 5 ? 1 : 0); }
 
-StepKernel pick_kernel(const FxKernelParams& P, int lean = -1) {
+// audit < 0: the variant for the current state of the bracket audit (P.audit)
+StepKernel pick_kernel(const FxKernelParams& P, int lean = -1, int audit = -1) {
   const int mode = kernel_mode(P, lean < 0 ? P.lean : lean);
   switch (P.cfg.strategy) {
     case FX_STRATEGY_DEFAULT: return pick_reward<FX_STRATEGY_DEFAULT>(P.cfg.reward, mode);
     case FX_STRATEGY_FIXED_SLTP: return pick_reward<FX_STRATEGY_FIXED_SLTP>(P.cfg.reward, mode);
-    default: return pick_reward<FX_STRATEGY_ATR_SLTP>(P.cfg.reward, mode);
+    default:
+      return (audit < 0 ? P.audit != nullptr : audit != 0) ? pick_reward<FX_KSTRAT_ATR_AUDIT>(P.cfg.reward, mode)
+                                                            : pick_reward<FX_STRATEGY_ATR_SLTP>(P.cfg.reward, mode);
   }
 }
 
-RolloutKernel pick_rollout(const FxKernelParams& P, int lean = -1) {
+RolloutKernel pick_rollout(const FxKernelParams& P, int lean = -1, int audit = -1) {
   const int mode = kernel_mode(P, lean < 0 ? P.lean : lean);
   const bool res = P.order_smem != 0;
   switch (P.cfg.strategy) {
     case FX_STRATEGY_DEFAULT: return pick_rollout_reward<FX_STRATEGY_DEFAULT>(P.cfg.reward, mode, res);
     case FX_STRATEGY_FIXED_SLTP: return pick_rollout_reward<FX_STRATEGY_FIXED_SLTP>(P.cfg.reward, mode, res);
-    default: return pick_rollout_reward<FX_STRATEGY_ATR_SLTP>(P.cfg.reward, mode, res);
+    default:
+      return (audit < 0 ? P.audit != nullptr : audit != 0) ? pick_rollout_reward<FX_KSTRAT_ATR_AUDIT>(P.cfg.reward, mode, res)
+                                                            : pick_rollout_reward<FX_STRATEGY_ATR_SLTP>(P.cfg.reward, mode, res);
   }
 }
 
@@ -1500,23 +1533,28 @@ cudaError_t fx_configure_kernels(FxKernelParams& P) {
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   P.num_sms = sms > 0 ? sms : 1;
   P.resident_blocks = 0;
-  // both the general and the LEAN instantiation: which one runs is only known once the candle tables are loaded
-  for (int lean = 0; lean <= (P.fast_features == 5 ? 1 : 0); lean++) {
-    cudaError_t e = cudaFuncSetAttribute(pick_kernel(P, lean), cudaFuncAttributePreferredSharedMemoryCarveout, pct);
+  // both the general and the LEAN instantiation: which one runs is only known once the candle tables are loaded; for
+  // the ATR strategy also both states of the bracket audit
+  const int n_lean = P.fast_features == 5 ? 2 : 1;
+  for (int v = 0; v < n_lean * (P.cfg.strategy == FX_STRATEGY_ATR_SLTP ? 2 : 1); v++) {
+    const int lean = v % n_lean, audit = v / n_lean;
+    cudaError_t e = cudaFuncSetAttribute(pick_kernel(P, lean, audit), cudaFuncAttributePreferredSharedMemoryCarveout, pct);
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(pick_rollout(P, lean), cudaFuncAttributePreferredSharedMemoryCarveout, rpct);
+    e = cudaFuncSetAttribute(pick_rollout(P, lean, audit), cudaFuncAttributePreferredSharedMemoryCarveout, rpct);
     if (e != cudaSuccess) return e;
     if (smem > 48 * 1024) {
-      e = cudaFuncSetAttribute(pick_kernel(P, lean), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      e = cudaFuncSetAttribute(pick_kernel(P, lean, audit), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return e;
     }
     if (rsmem > 48 * 1024) {
-      e = cudaFuncSetAttribute(pick_rollout(P, lean), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rsmem);
+      e = cudaFuncSetAttribute(pick_rollout(P, lean, audit), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rsmem);
       if (e != cudaSuccess) return e;
     }
-    // how many CTAs of the persistent rollout kernel the device holds at once (= its grid size)
+    // how many CTAs of the persistent rollout kernel the device holds at once (= its grid size).  The minimum over every
+    // variant configured here, the bracket audit's included: one grid size serves whichever variant a launch picks, so a
+    // change that raises the audit kernels' registers or shared memory shrinks the grid with the log off as well
     int per_sm = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pick_rollout(P, lean), rcta * 32, rsmem);
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pick_rollout(P, lean, audit), rcta * 32, rsmem);
     if (e != cudaSuccess) return e;
     if (P.resident_blocks == 0 || sms * per_sm < P.resident_blocks) P.resident_blocks = sms * per_sm;
   }

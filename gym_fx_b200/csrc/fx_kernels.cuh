@@ -77,6 +77,11 @@ struct FxKernelParams {
   int32_t lean;             // 1: the configuration qualifies for the specialised kernels (fx_config_is_lean)
   int32_t num_sms;          // SMs of the device (fx_rollout_kernel: CTA b is the (b / num_sms)-th CTA of its SM)
   int32_t order_smem;       // 1: fx_rollout_kernel keeps each ticket's order table in shared memory (fx_order_smem_choice)
+  // bracket audit (fxenv_set_bracket_audit): [N][audit_cap][FXENV_AU_FIELDS] ring and [N] record counters, or nullptr
+  // (log off).  Outside the state slab: snapshots and the slab layout do not depend on the log.
+  double* audit;
+  int64_t* audit_written;
+  int32_t audit_cap;
 };
 
 // warps (= envs) per CTA of the step kernel.  One warp per CTA lets the second wave back-fill SM slots as soon as a

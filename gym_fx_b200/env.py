@@ -11,6 +11,9 @@ Differences, all deliberate (SURVEY.md App. B):
     ignores include_price_window/include_agent_state, App. B #9);
   * there is no backtrader: `summary()` passes an empty analyzers dict to the metrics plugin, which is what the
     reference effectively does on the live path (App. B #12).
+
+With direct_atr_sltp and GYMFX_BRACKET_AUDIT set (read at import of the strategy module, as in the reference), every
+step() appends the decisions the step kernel logged to that file, in the reference's line format.
 """
 from __future__ import annotations
 
@@ -20,7 +23,8 @@ import numpy as np
 import torch
 
 from . import spaces
-from .config import lower_config, obs_layout
+from .config import STRATEGY_ATR_SLTP, lower_config, obs_layout
+from .strategy_plugins import direct_atr_sltp as _atr
 from .vec_env import VecFxEnv
 
 
@@ -96,6 +100,8 @@ class GymFxEnv(spaces.EnvBase):
             self._np_random = np.random.default_rng(seed)  # unused by the dynamics, as in the reference
         if self._vec is None:
             self._vec = VecFxEnv(self._fxcfg, [self._table], [self._minutes])
+            if _atr._AUDIT_PATH and self._fxcfg.strategy == STRATEGY_ATR_SLTP:
+                self._vec.set_bracket_audit(4)  # at most one record per step, drained after every step
         obs, _ = self._vec.reset(torch.zeros(1, dtype=torch.int64))
         self._started = True
         self._terminated = False
@@ -110,6 +116,8 @@ class GymFxEnv(spaces.EnvBase):
         was_terminated = self._terminated
         a = torch.tensor([self._host_action(action)], dtype=self._vec.action_dtype, device=self._vec.device)
         obs, _, term, _, _ = self._vec.step(a)
+        if self._vec._audit is not None:
+            self._emit_audit()
         reward = float(self._vec.reward64[0])          # fp64, like the reference's Python float
         terminated = bool(term[0])
         self._terminated = terminated
@@ -144,6 +152,13 @@ class GymFxEnv(spaces.EnvBase):
         except Exception:
             a = 0
         return a if -2**31 <= a < 2**31 else 0
+
+    def _emit_audit(self):
+        """_audit_emit (strategy_plugins/direct_atr_sltp.py:35-45) for the records of the last step."""
+        r = self._vec.bracket_audit()
+        if r["kind"].numel() and _atr._AUDIT_PATH:
+            cols = [r[k].tolist() for k in ("kind", "entry", "stop", "limit", "size", "atr")]
+            _atr.audit_append(_atr._AUDIT_PATH, "".join(_atr.audit_line(*rec) for rec in zip(*cols)))
 
     def _split(self, row: np.ndarray) -> Dict[str, np.ndarray]:
         return {k: row[off:off + int(np.prod(shape))].reshape(shape).copy() for k, (off, shape) in self._layout.items()}

@@ -63,6 +63,7 @@ class VecFxEnv:
         self._info_views: Dict[str, torch.Tensor] = {}
         self.action_dtype = torch.float32 if cfg.action_mode == 1 else torch.int32
         self._policies: list = []
+        self._audit = None  # (ring [N, capacity, 8], written [N], read cursor [N]) while the bracket audit is on
 
     # ------------------------------------------------------------------ lifecycle
     def close(self):
@@ -70,6 +71,7 @@ class VecFxEnv:
             # the info tensors are zero-copy views of the library's state slab, which fxenv_destroy frees: drop the cached
             # ones (views a caller still holds become invalid, like any tensor handed out by info() -- clone to keep)
             self._info_views.clear()
+            self._audit = None
             for pol in list(getattr(self, "_policies", [])):   # policies hold device buffers tied to this handle
                 pol.close()
             self.L.fxenv_destroy(self._h)
@@ -358,6 +360,55 @@ class VecFxEnv:
             "avg_trade_pnl": torch.where(closed > 0, col["pnl_net"] / closed.clamp(min=1.0), nan),
             "sqn": self._sqn(col["pnl_net"], col["pnl_sq"], closed), "episode_index": col["index"].to(torch.int64),
         }
+
+    # ------------------------------------------------------------------ bracket audit
+    def set_bracket_audit(self, capacity: int):
+        """Turn the ATR strategy's bracket audit on with a ring of `capacity` records per env (the counters and the read
+        cursors restart at 0), or off with 0 (include/fxenv.h fxenv_set_bracket_audit).  Accepted for every strategy;
+        only direct_atr_sltp writes records.  Synchronous."""
+        capacity = int(capacity)
+        if not 0 <= capacity < 2**31:
+            raise ValueError(f"bracket audit capacity must be in [0, 2**31), got {capacity}")
+        with torch.cuda.device(self.device):
+            rc = self.L.fxenv_set_bracket_audit(self._h, capacity)
+        if rc == -1:
+            raise ValueError(self.L.fxenv_last_error(self._h).decode())
+        _native.check(self.L, self._h, rc, "fxenv_set_bracket_audit")
+        self._audit = None
+        if capacity:
+            p = _native.FxAuditPtrs()
+            _native.check(self.L, self._h, self.L.fxenv_get_bracket_audit(self._h, C.byref(p)), "fxenv_get_bracket_audit")
+            N, F = self.num_envs, _native.AU_FIELDS
+            ring = _tensor_from_ptr(p.records, N * p.capacity * F, torch.float64, self.device).view(N, p.capacity, F)
+            written = _tensor_from_ptr(p.written, N, torch.int64, self.device)
+            self._audit = (ring, written, torch.zeros(N, dtype=torch.int64, device=self.device))
+
+    def bracket_audit(self) -> Dict[str, torch.Tensor]:
+        """Drain the audit rings: every record written since the last drain, as device tensors ordered by env and then
+        by record -- env, bar (table row of the signal bar), episode (the episode's k), kind (1 long_bracket, 2
+        short_bracket, 3 session_force_close), entry, stop, limit, size, atr (NaN stop / limit / atr for a force-close) --
+        plus dropped [N]: records overwritten in the ring before they could be drained.  Ordered on the current stream
+        (torch ops; sizing the result waits for the counters).  The log must be on (set_bracket_audit)."""
+        if getattr(self, "_audit", None) is None:
+            raise _native.FxEnvError("the bracket audit is off: call set_bracket_audit(capacity) first")
+        ring, written, cursor = self._audit
+        N, cap = self.num_envs, ring.shape[1]
+        w = written.clone()
+        first = torch.maximum(cursor, w - cap)
+        dropped = first - cursor
+        count = w - first
+        env = torch.repeat_interleave(torch.arange(N, device=self.device), count)
+        offset = torch.cumsum(count, 0) - count
+        idx = first[env] + (torch.arange(env.numel(), device=self.device) - offset[env])
+        rec = ring[env, idx % cap]
+        cursor.copy_(w)
+        A = _native.AU
+        out = {"env": env, "bar": rec[:, A["bar"]].to(torch.int64), "episode": rec[:, A["episode"]].to(torch.int64),
+               "kind": rec[:, A["kind"]].to(torch.int32)}
+        for k in ("entry", "stop", "limit", "size", "atr"):
+            out[k] = rec[:, A[k]]
+        out["dropped"] = dropped
+        return out
 
     # ------------------------------------------------------------------ closed loop (policy on the device)
     def make_policy(self, weights=None) -> "FusedPolicy":

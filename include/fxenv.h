@@ -280,6 +280,45 @@ typedef struct FxEpisodePtrs {
 
 int fxenv_get_episode_info(FxEnv* env, FxEpisodePtrs* out);
 
+/* ---- bracket audit: the GYMFX_BRACKET_AUDIT log of direct_atr_sltp (strategy_plugins/direct_atr_sltp.py:35-45,
+ * :138-142, :188-191, :199-202) -----------------------------------------------------------------------------------
+ * With the log on, every env-step of the ATR strategy that the reference would log writes one record of
+ * FXENV_AU_FIELDS doubles into a per-env ring of `capacity` records:
+ *   long_bracket / short_bracket: action 1 / 2 once the session entry check and the ready / atr > 0 / size > 0 /
+ *     close > 0 checks pass, and only when the position is <= 0 / >= 0 (a short / long is closed first, same call);
+ *   session_force_close: the bar is in the close zone and the position is non-zero, whatever the action.
+ * A record is written whether or not its orders later fill or are rejected, and also when the order table had no room
+ * for them (FX_FLAG_ORDER_OVERFLOW drops the orders, the reference's unbounded list would have taken them).  At most one
+ * record per env-step; records of one env stay in call order.  The other strategies write nothing.
+ * written[i] counts env i's records since the log was enabled; record j of env i sits at
+ * records[(i * capacity + j % capacity) * FXENV_AU_FIELDS].  The ring and the counters live outside the env state:
+ * fxenv_state_bytes and snapshots do not include them, and fxenv_reset / fxenv_set_state leave them alone. */
+#define FXENV_AU_FIELDS 8
+enum {
+  FXENV_AU_KIND = 0,   /* FXENV_AU_KIND_* */
+  FXENV_AU_BAR,        /* table row of the signal bar (start + t) */
+  FXENV_AU_EPISODE,    /* the episode's k (FXENV_EP_INDEX) */
+  FXENV_AU_ENTRY,      /* close of the signal bar */
+  FXENV_AU_STOP,       /* stop price passed to buy_bracket / sell_bracket (NaN for a force-close) */
+  FXENV_AU_LIMIT,      /* limit price (NaN for a force-close) */
+  FXENV_AU_SIZE,       /* _compute_size; for a force-close the signed position before the close fills */
+  FXENV_AU_ATR         /* simple-mean ATR (NaN for a force-close) */
+};
+enum { FXENV_AU_KIND_NONE = 0, FXENV_AU_KIND_LONG = 1, FXENV_AU_KIND_SHORT = 2, FXENV_AU_KIND_FORCE_CLOSE = 3 };
+
+/* capacity > 0: (re)allocates the ring for capacity records per env and zeroes the counters (log on); 0: frees it (log
+ * off); < 0 or too large: FXENV_E_INVALID.  Accepted for every strategy.  Synchronous. */
+int fxenv_set_bracket_audit(FxEnv* env, int32_t capacity);
+
+/* Device pointers of the log, valid until the next fxenv_set_bracket_audit / fxenv_destroy; all NULL / 0 when off. */
+typedef struct FxAuditPtrs {
+  const double* records;    /* [num_envs][capacity][FXENV_AU_FIELDS] */
+  const int64_t* written;   /* [num_envs] */
+  int32_t capacity;
+} FxAuditPtrs;
+
+int fxenv_get_bracket_audit(FxEnv* env, FxAuditPtrs* out);
+
 /* ---- closed loop: a policy on the device between the steps ------------------------------------------------------
  * Replaces the caller loop of app/main.py:57-65 (`action = strategy.decide_action(obs, info, step); env.step(action)`)
  * for a learned actor-critic (BASELINE configs[3]: PPO MLP(256,256)): observation rows never leave the GPU, and the
