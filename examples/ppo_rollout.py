@@ -11,6 +11,7 @@ minibatch and advantages are normalised with global statistics (gym_fx_b200.lear
     python examples/ppo_rollout.py --envs 4096 --horizon 32 --updates 5
     python examples/ppo_rollout.py --envs 4096 --action-space continuous --updates 5 --eval-rollouts 2
     python examples/ppo_rollout.py --envs 4096 --episode-bars 500 --holdout-frac 0.2 --eval-rollouts 2
+    python examples/ppo_rollout.py --envs 4096 --action-repeat 5 --repeat-mode hold
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 examples/ppo_rollout.py --envs 4096
 
 --action-space continuous trains a Gaussian actor on the Box(-1, 1) action (thresholded to hold / long / short by the
@@ -21,7 +22,10 @@ draws a new one, VecFxEnv.set_episode_starts), and the greedy evaluation resets 
 episode records (VecFxEnv.episode_stats) then give, for training and for evaluation, the episodes finished and the mean
 total return and maximum drawdown of each env's last finished episode (the reset into the tail, and one after the
 evaluation, record the episodes they cut short).
-Prints one JSON line: env-steps/s of the rollout phase (policy in the loop) and of the whole train loop.
+--action-repeat K lets the policy decide once per K bars (VecFxEnv.set_action_repeat): a rollout step is a decision,
+GAE runs per decision.  --repeat-mode repeat applies the action on every bar of the step, hold on its first bar only.
+Prints one JSON line: env-steps/s (decisions) of the rollout phase (policy in the loop) and of the whole train loop, and
+bars/s of the rollout phase as an upper bound (decisions x K: a step that ends an episode runs fewer bars).
 """
 from __future__ import annotations
 
@@ -52,12 +56,17 @@ def main():
     ap.add_argument("--episode-bars", type=int, default=0, help="bars per episode (0: an episode runs to the end of the table)")
     ap.add_argument("--holdout-frac", type=float, default=0.0,
                     help="fraction of every table held out of training for the greedy evaluation (needs --episode-bars)")
+    ap.add_argument("--action-repeat", type=int, default=1, help="bars per decision (1..256)")
+    ap.add_argument("--repeat-mode", choices=("repeat", "hold"), default="repeat",
+                    help="repeat: the action on every bar of a step; hold: on its first bar, then hold")
     args = ap.parse_args()
     continuous = args.action_space == "continuous"
     if not 0.0 <= args.holdout_frac < 1.0:
         ap.error("--holdout-frac must be in [0, 1)")
     if args.holdout_frac > 0.0 and args.episode_bars <= 0:
         ap.error("--holdout-frac needs --episode-bars (an episode must fit inside its part of the table)")
+    if not 1 <= args.action_repeat <= 256:
+        ap.error("--action-repeat must be in 1..256")
 
     import bench
     from gym_fx_b200.learner import ActorCritic, ppo_update
@@ -83,7 +92,10 @@ def main():
         desc += f", episodes of {args.episode_bars} bars"
     env = VecFxEnv(cfg, candles, minutes, device=dev)
     check_pair_alignment(N, cfg.num_pairs)
-    H = args.horizon
+    H, K = args.horizon, args.action_repeat
+    if K > 1:
+        env.set_action_repeat(K, hold=args.repeat_mode == "hold")
+        desc += f", one decision per {K} bars ({args.repeat_mode})"
     T, L = bench.T_BARS, args.episode_bars
     split = int(T * (1.0 - args.holdout_frac))       # training bars [0, split), held-out bars [split, T)
     if args.holdout_frac > 0.0:
@@ -93,7 +105,7 @@ def main():
         env.set_episode_starts(0, split - L, seed=0x5EED0000 + rank)   # a window [start, start + L) inside training
         env.reset()
     else:
-        env.reset(torch.as_tensor(shard_starts(N, rank, world, T, (args.updates + args.eval_rollouts + 2) * H + 64, 256)))
+        env.reset(torch.as_tensor(shard_starts(N, rank, world, T, (args.updates + args.eval_rollouts + 2) * H * K + 64, 256)))
 
     torch.backends.cuda.matmul.allow_tf32 = True
     torch.manual_seed(0)  # identical replicas on every rank
@@ -166,6 +178,8 @@ def main():
             "policy": f"MLP({D},256,256) actor-critic ({args.action_space} actions), fused wgmma kernel in the rollout, "
                       "torch (tf32) in the update",
             "rollout_env_steps_per_s": steps / max(t_roll, 1e-9), "rollout_us_per_step": t_roll / (H * n_it) * 1e6,
+            "action_repeat": K, "repeat_mode": args.repeat_mode,
+            "rollout_bars_per_s_upper_bound": steps * K / max(t_roll, 1e-9),
             "train_env_steps_per_s": steps / max(t_roll + t_upd, 1e-9), "update_s": t_upd / n_it, **stats}), flush=True)
     env.close()
     if dist:

@@ -31,11 +31,12 @@ EXPORTS = [
     "fxenv_state_bytes", "fxenv_get_state", "fxenv_set_state", "fxenv_launch_count", "fxenv_step_many_engine",
     "fxenv_policy_create", "fxenv_policy_set_weights", "fxenv_policy_destroy", "fxenv_rollout", "fxenv_policy_sync_timeouts",
     "fxenv_rollout_ex", "fxenv_policy_peek", "fxenv_set_reset_starts", "fxenv_get_episode_info",
-    "fxenv_set_bracket_audit", "fxenv_get_bracket_audit",
+    "fxenv_set_bracket_audit", "fxenv_get_bracket_audit", "fxenv_set_action_repeat",
 ]
 
 ROLLOUT_GREEDY = 1  # FXENV_ROLLOUT_GREEDY
 PEEK_OBS16, PEEK_H1 = 0, 1  # FXENV_PEEK_*
+MAX_REPEAT, REPEAT_HOLD = 256, 1  # FXENV_MAX_REPEAT, FXENV_REPEAT_HOLD
 
 
 class FxEnvError(RuntimeError):
@@ -140,6 +141,7 @@ def load():
     L.fxenv_get_episode_info.argtypes = [vp, C.POINTER(FxEpisodePtrs)]
     L.fxenv_set_bracket_audit.argtypes = [vp, C.c_int32]
     L.fxenv_get_bracket_audit.argtypes = [vp, C.POINTER(FxAuditPtrs)]
+    L.fxenv_set_action_repeat.argtypes = [vp, C.c_int32, C.c_uint32]
     if L.fxenv_abi_version() != 2:
         raise FxEnvError("libfxenv.so ABI version mismatch")
     _lib = L

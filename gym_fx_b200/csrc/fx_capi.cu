@@ -65,8 +65,9 @@ struct FxEnv {
     uint64_t used = 0;
   } graphs[2];
   uint64_t graph_clock = 0;
-  // bumped whenever P.audit / audit_cap change: a cached rollout graph captured the old P by value (FxPolicy::cached)
-  uint64_t audit_epoch = 0;
+  // bumped whenever a setting in the kernel parameters changes (the bracket audit, the action repeat): a cached rollout
+  // graph captured the old P by value (FxPolicy::cached)
+  uint64_t params_epoch = 0;
 };
 
 namespace {
@@ -172,6 +173,7 @@ int fxenv_create(const FxConfig* cfg, FxEnv** out) {
   env->P.cap = cap;
   env->P.obs_dim = (int32_t)fx_obs_dim(c);
   env->P.inv_initial_cash = 1.0 / (c.initial_cash != 0.0 ? c.initial_cash : 1.0);
+  env->P.repeat = 1;  // no action repeat (fxenv_set_action_repeat)
   if (const char* dv = getenv("FXENV_DEBUG")) env->P.debug = atoi(dv);  // timing experiments only
   if (const char* tv = getenv("FXENV_TIMING")) {
     if (atoi(tv)) {
@@ -607,7 +609,7 @@ int fxenv_set_bracket_audit(FxEnv* env, int32_t capacity) {
   DeviceGuard g(env->device);
   FX_CUDA(env, cudaDeviceSynchronize());  // kernels in flight may still write the old ring
   drop_graph(env);                        // the cached step-many graphs captured the old P
-  env->audit_epoch++;                     // ... and so did each policy's rollout graph (re-captured on its next use)
+  env->params_epoch++;                    // ... and so did each policy's rollout graph (re-captured on its next use)
   cudaFree(env->P.audit); cudaFree(env->P.audit_written);
   env->P.audit = nullptr; env->P.audit_written = nullptr; env->P.audit_cap = 0;
   if (capacity == 0) return FXENV_OK;
@@ -626,6 +628,21 @@ int fxenv_set_bracket_audit(FxEnv* env, int32_t capacity) {
 int fxenv_get_bracket_audit(FxEnv* env, FxAuditPtrs* out) {
   if (!env || !out) return FXENV_E_INVALID;
   out->records = env->P.audit; out->written = env->P.audit_written; out->capacity = env->P.audit_cap;
+  return FXENV_OK;
+}
+
+int fxenv_set_action_repeat(FxEnv* env, int32_t repeat, uint32_t flags) {
+  if (!env) return FXENV_E_INVALID;
+  if (repeat < 1 || repeat > FXENV_MAX_REPEAT)
+    return fail(env, FXENV_E_INVALID, "action repeat must be in 1.." + std::to_string(FXENV_MAX_REPEAT) + ", got " + std::to_string(repeat));
+  if (flags & ~FXENV_REPEAT_HOLD) return fail(env, FXENV_E_INVALID, "unknown action repeat flags " + std::to_string(flags));
+  if (repeat == env->P.repeat && flags == env->P.repeat_flags) return FXENV_OK;
+  DeviceGuard g(env->device);
+  FX_CUDA(env, cudaDeviceSynchronize());  // no cached graph is destroyed while a launch of it may be running
+  drop_graph(env);       // the cached step-many graphs captured the old P
+  env->params_epoch++;   // ... and so did each policy's rollout graph
+  env->P.repeat = repeat;
+  env->P.repeat_flags = flags;
   return FXENV_OK;
 }
 
@@ -706,7 +723,7 @@ struct FxPolicy {
   FxPolicyDev dev;
   bool has_weights = false;
   bool continuous = false;             // FX_ACTION_CONTINUOUS: Gaussian head, float32 actions (fx_policy_kernel<true>)
-  struct { cudaGraphExec_t exec = nullptr; FxRollout io; uint32_t flags = 0; uint64_t audit_epoch = 0; } cached;
+  struct { cudaGraphExec_t exec = nullptr; FxRollout io; uint32_t flags = 0; uint64_t params_epoch = 0; } cached;
 };
 
 namespace {
@@ -950,7 +967,7 @@ int fxenv_rollout_ex(FxEnv* env, FxPolicy* pol, const FxRollout* io, uint32_t fl
   // the graph bakes in the buffers, the seed, the flags (greedy or sampling) and the env's kernel parameters (P, by
   // value: the bracket audit ring): any change re-captures it
   if (!pol->cached.exec || memcmp(&pol->cached.io, io, sizeof(FxRollout)) != 0 || pol->cached.flags != flags ||
-      pol->cached.audit_epoch != env->audit_epoch) {
+      pol->cached.params_epoch != env->params_epoch) {
     if (pol->cached.exec) { cudaGraphExecDestroy(pol->cached.exec); pol->cached.exec = nullptr; }
     cudaGraph_t graph = nullptr;
     FX_CUDA(env, cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
@@ -963,7 +980,7 @@ int fxenv_rollout_ex(FxEnv* env, FxPolicy* pol, const FxRollout* io, uint32_t fl
     if (e != cudaSuccess) { pol->cached.exec = nullptr; return cuda_fail(env, e, "cudaGraphInstantiate"); }
     pol->cached.io = *io;
     pol->cached.flags = flags;
-    pol->cached.audit_epoch = env->audit_epoch;
+    pol->cached.params_epoch = env->params_epoch;
   }
   FX_CUDA(env, cudaGraphLaunch(pol->cached.exec, stream));
   env->launches += nl;

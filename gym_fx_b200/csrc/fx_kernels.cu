@@ -704,27 +704,44 @@ __device__ __noinline__ void fx_audit_store(const FxKernelParams& P, const int e
   if (lane == 0) P.audit_written[env] = (int64_t)(w + 1);
 }
 
+// Action repeat (include/fxenv.h, fxenv_set_action_repeat): kernel template STRAT + FX_KSTRAT_REPEAT is the strategy STRAT
+// with a step of up to P.repeat substeps.  The host launches these instantiations only while k > 1, so with k = 1 the
+// kernels are exactly those of a build without the repeat.  One fx_step_env call runs one substep; this record is what the
+// substeps of one step share.
+#define FX_KSTRAT_REPEAT 4
+struct FxSubstep {
+  double racc;  // float64 sum of the rewards of the step's substeps so far
+  int j;        // index of this substep
+  bool ended;   // out: this substep ended the step (the last one, a terminating one, or the step of a terminated env)
+};
+
 // One env-step of one env by one warp (everything between the cross-kernel dependency wait and the release).
 // CARRY (fx_rollout_kernel): the step leaves the env's scalar state in ws.carry and returns true if that record is valid;
 // carry_in = the previous call of this warp was the same env's previous step and returned true.
 // RESIDENT (with CARRY): the env's order table lives in ws.op0/op1/osz/ometa while the carry record is valid -- loaded
 // from global memory by a step without carry_in, written back by a step that returns false (terminated branch) and by
 // the caller at the end of its ticket (fx_rollout_kernel).
+// REPEAT (STRAT >= FX_KSTRAT_REPEAT, with CARRY): the call is substep sub->j of a step.  A substep that does not end the
+// step issues no window copy, stages no statistics and stores no row, reward or flag (the running Welford statistics
+// still advance); it adds its reward to sub->racc and leaves the carry record for the next substep.
 template <int STRAT, int REWARD, bool FAST5, bool O16, bool LEAN, bool CARRY = false, bool RESIDENT = false>
 __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void* __restrict__ actions, float* __restrict__ obs,
                                             float* __restrict__ reward, double* __restrict__ reward64,
                                             uint8_t* __restrict__ terminated, const int env, const int lane, const WarpSmem& ws,
                                             const unsigned phase = 0u, const unsigned step_row = 0u, const unsigned obs_slot_row = 0u,
                                             uint16_t* __restrict__ obs16 = nullptr, const int stride16 = 0,
-                                            const bool carry_in = false) {
+                                            const bool carry_in = false, FxSubstep* sub = nullptr) {
   // `actions` / `reward` / `terminated` / `obs` are the BASES of the caller's arrays (kernel parameters: they cost no
   // registers); this env-step's element is at index step_row + env (step_row = step * num_envs) and its observation row
   // at obs_slot_row + env (obs_slot_row = slot * num_envs).  Addresses are formed where they are used.
 #define FX_OBS_ROW() (obs + ((size_t)obs_slot_row + (size_t)env) * (size_t)P.obs_dim)
 #define FX_OUT_IDX() ((size_t)step_row + (size_t)env)
 #define FX_OBS_ROW16() ((O16 && obs16) ? obs16 + (size_t)env * (size_t)stride16 : nullptr)  // bf16 copy (single-step kernel only)
-  constexpr bool ATR = STRAT == FX_STRATEGY_ATR_SLTP || STRAT == FX_KSTRAT_ATR_AUDIT;
-  constexpr int STRATEGY = ATR ? FX_STRATEGY_ATR_SLTP : STRAT;  // what fx_apply_action runs
+  constexpr bool REPEAT = STRAT >= FX_KSTRAT_REPEAT;
+  constexpr int KSTRAT = REPEAT ? STRAT - FX_KSTRAT_REPEAT : STRAT;
+  constexpr bool ATR = KSTRAT == FX_STRATEGY_ATR_SLTP || KSTRAT == FX_KSTRAT_ATR_AUDIT;
+  constexpr int STRATEGY = ATR ? FX_STRATEGY_ATR_SLTP : KSTRAT;  // what fx_apply_action runs
+  static_assert(!REPEAT || CARRY, "substeps hand the env over through the carry record");
   const FxConfig& c = P.cfg;
   const FxDeviceState& st = P.st;
   const int C = c.n_cols;
@@ -854,6 +871,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       fx_window_wait(ws, phase);
       fx_emit_windows<FAST5, O16, LEAN>(P, lane, s, scale, ws.win + shift, ws.stat, FX_OBS_ROW(), FX_OBS_ROW16());
     }
+    if (REPEAT) sub->ended = true;  // rule 1 of the repeat: a terminated env runs this one substep
     return false;  // (the carry record does not follow resets / ended episodes: the next step reloads the arrays)
   }
 
@@ -886,8 +904,12 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   int win_left = s_obs - c.window_size;
   if (win_left < 0) win_left = 0;
   int win_shift = 0;
+  // REPEAT: only the step's last substep is known to emit here; one that ends the step by terminating emits as well, and
+  // issues its copy then (cold path).  Without the repeat every call emits.
+  const bool last_sub = !REPEAT || sub->j + 1 >= P.repeat;
+  bool emit = last_sub;
   __syncwarp();
-  if (!(dbg & 1))  // the observation window and (steady state) the bar's z-score statistics: TMA -> shared memory
+  if (!(dbg & 1) && last_sub)  // the observation window and (steady state) the bar's z-score statistics: TMA -> shared memory
     win_shift = fx_window_issue(tb, C, start, win_left, s_obs - win_left, lane, ws,
                                 table_stats ? tb.stats + (start + t) * (int64_t)c.n_features * 2 : nullptr, c.n_features);
 
@@ -900,21 +922,26 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   // extra round trip here instead of registers held across the broker pass.
 #define FX_EMIT_OBSERVATION()                                                                              \
   do {                                                                                                     \
-    if (lane < c.n_features && (welford_live || (scale && !table_stats))) {                                \
+    if (REPEAT && emit && !last_sub && !(dbg & 1)) {                                                       \
+      __syncwarp();                                                                                        \
+      win_shift = fx_window_issue(tb, C, start, win_left, s_obs - win_left, lane, ws,                      \
+                                  table_stats ? tb.stats + (start + t) * (int64_t)c.n_features * 2 : nullptr, c.n_features); \
+    }                                                                                                      \
+    if (lane < c.n_features && (welford_live || ((!REPEAT || emit) && scale && !table_stats))) {           \
       const int64_t wi = ((int64_t)env * FXENV_MAX_FEATURES + lane) * 2;                                   \
       double wf_m = st.welford[wi], wf_m2 = st.welford[wi + 1];                                            \
       if (welford_live) {                                                                                  \
         fx_welford_step(wf_m, wf_m2, row[c.feature_cols[lane]], t + 1);                                    \
         st.welford[wi] = wf_m; st.welford[wi + 1] = wf_m2;                                                 \
       }                                                                                                    \
-      if (scale && !table_stats) {                                                                         \
+      if ((!REPEAT || emit) && scale && !table_stats) {                                                    \
         double st_m, st_r;                                                                                 \
         fx_welford_to_stats(wf_m, wf_m2, hn, st_m, st_r);                                                  \
         ws.stat[2 * lane] = st_m; ws.stat[2 * lane + 1] = st_r;                                            \
       }                                                                                                    \
     }                                                                                                      \
     __syncwarp();                                                                                          \
-    if (!(dbg & 1)) {                                                                                      \
+    if ((!REPEAT || emit) && !(dbg & 1)) {                                                                 \
       fx_window_wait(ws, phase);                                                                           \
       fx_emit_windows<FAST5, O16, LEAN>(P, lane, s_obs, scale, ws.win + win_shift, ws.stat, FX_OBS_ROW(), FX_OBS_ROW16()); \
     }                                                                                                      \
@@ -1043,8 +1070,11 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
     int n_final = n_live, n_acc_new = n_live;
     double sub_need_new = 0.0;
     if (!exhausted) {
-      const int action = (!LEAN && c.action_mode == FX_ACTION_CONTINUOUS) ? fx_coerce_continuous(c, action_raw_f)
-                                                                           : fx_coerce_discrete(action_raw_i);
+      // hold mode: the substeps after the first run the coerced hold action 0 itself
+      const bool hold = REPEAT && sub->j > 0 && (P.repeat_flags & FXENV_REPEAT_HOLD);
+      const int action = hold ? 0
+                              : (!LEAN && c.action_mode == FX_ACTION_CONTINUOUS) ? fx_coerce_continuous(c, action_raw_f)
+                                                                                  : fx_coerce_discrete(action_raw_i);
       double atr = 0.0;
       bool atr_ready = false;
       if (ATR && action != 0) {
@@ -1080,7 +1110,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       FxAudit au;
       au.kind = FXENV_AU_KIND_NONE;
       fx_apply_action(c, STRATEGY, e, tg, action, b, pair, atr, atr_ready, has_min, minutes, au);
-      if (STRAT == FX_KSTRAT_ATR_AUDIT && au.kind != FXENV_AU_KIND_NONE) fx_audit_store(P, env, lane, au, start + t, b.c);
+      if (KSTRAT == FX_KSTRAT_ATR_AUDIT && au.kind != FXENV_AU_KIND_NONE) fx_audit_store(P, env, lane, au, start + t, b.c);
       n_final = tg.n;
       sub_need_new = tg.sub_need;
       fx_publish(e, b.c, t);
@@ -1133,6 +1163,11 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       }
     }
     const bool term = ((e.flags & FX_FLAG_TERMINATED) != 0u) || (e.equity <= c.min_equity);  // app/env.py:157
+    if (REPEAT) {  // the step's reward: the substeps' sum in substep order, from r0; a terminating substep ends the step
+      if (sub->j > 0) r = sub->racc + r;
+      sub->racc = r;
+      emit = emit || term;
+    }
     FX_STAMP(7);  // reward
 
     // ---- write back (lane 0): always-changing columns, then the ones a fill touched
@@ -1147,10 +1182,12 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       if (n_final != n) st.n_orders[env] = n_final;
       if (n_acc_new != n_acc) st.n_acc[env] = n_acc_new;
       if (sub_need_new != sub_need) st.sub_need[env] = sub_need_new;
-      reward[FX_OUT_IDX()] = (float)r;
-      if (reward64) reward64[FX_OUT_IDX()] = r;
-      terminated[FX_OUT_IDX()] = term ? 1 : 0;
-      fx_write_scalars<LEAN>(P, e, total_bars, last_price, FX_OBS_ROW(), FX_OBS_ROW16());
+      if (!REPEAT || emit) {
+        reward[FX_OUT_IDX()] = (float)r;
+        if (reward64) reward64[FX_OUT_IDX()] = r;
+        terminated[FX_OUT_IDX()] = term ? 1 : 0;
+        fx_write_scalars<LEAN>(P, e, total_bars, last_price, FX_OBS_ROW(), FX_OBS_ROW16());
+      }
       if (CARRY) {  // what the env's next step starts from, should this warp run it (the arrays above stay authoritative)
         double* __restrict__ cr = ws.carry;
         cr[FX_CARRY_CASH] = e.cash; cr[FX_CARRY_PSIZE] = e.psize; cr[FX_CARRY_PPRICE] = e.pprice; cr[FX_CARRY_EQUITY] = e.equity;
@@ -1184,6 +1221,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
     if (lane < FX_RS_N) ws.carry[FX_CARRY_RSTATS + lane] = rsv;
 #endif
   }
+  if (REPEAT) sub->ended = emit;
   FX_STAMP(9);
   FX_STAMP_GLOBAL(11);
 #undef FX_EMIT_OBSERVATION
@@ -1194,6 +1232,29 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
 #undef FX_STAMP_DEP
 #undef FX_STAMP_GLOBAL
   return CARRY && !(dbg & 2);
+}
+
+// One step of up to P.repeat substeps (the REPEAT instantiations): substeps run until one ends the step.  They hand the
+// env to each other through the carry record (RESIDENT: and the shared copy of the order table), so only the first one
+// loads it from global memory.  Returns what the last substep returned.
+template <int STRAT, int REWARD, bool FAST5, bool O16, bool LEAN, bool RESIDENT>
+__device__ __forceinline__ bool fx_step_repeat(const FxKernelParams& P, const void* __restrict__ actions, float* __restrict__ obs,
+                                               float* __restrict__ reward, double* __restrict__ reward64,
+                                               uint8_t* __restrict__ terminated, const int env, const int lane, const WarpSmem& ws,
+                                               const unsigned phase, const unsigned step_row, const unsigned obs_slot_row,
+                                               uint16_t* __restrict__ obs16, const int stride16, bool carry) {
+  FxSubstep sub;
+  sub.racc = 0.0;
+  sub.ended = false;
+#pragma unroll 1
+  for (sub.j = 0;; ++sub.j) {
+    carry = fx_step_env<STRAT, REWARD, FAST5, O16, LEAN, true, RESIDENT>(P, actions, obs, reward, reward64, terminated, env, lane,
+                                                                       ws, phase, step_row, obs_slot_row, obs16, stride16,
+                                                                       carry, &sub);
+    if (sub.ended) break;
+    __syncwarp();  // the substep's stores (state arrays, carry record) before the next substep's loads
+  }
+  return carry;
 }
 
 __device__ __forceinline__ int fx_ld_acquire(const int32_t* p) {
@@ -1254,8 +1315,13 @@ fx_step_kernel(const __grid_constant__ FxKernelParams P, const void* __restrict_
   if (klog) { long long g1; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g1)); klog[2] = g1; }
 #endif
   // the bf16 copy of the row (closed loop only) is a compile-time variant: no per-store pointer tests in the plain step
-  if (obs16) fx_step_env<STRAT, REWARD, FAST5, true, LEAN>(P, actions, obs, reward, reward64, terminated, env, lane, ws, 0u, 0u, 0u, obs16, stride16);
-  else fx_step_env<STRAT, REWARD, FAST5, false, LEAN>(P, actions, obs, reward, reward64, terminated, env, lane, ws);
+  if constexpr (STRAT >= FX_KSTRAT_REPEAT) {  // action repeat: the step's substeps (the emitting one writes both rows)
+    if (obs16) fx_step_repeat<STRAT, REWARD, FAST5, true, LEAN, false>(P, actions, obs, reward, reward64, terminated, env, lane, ws, 0u, 0u, 0u, obs16, stride16, false);
+    else fx_step_repeat<STRAT, REWARD, FAST5, false, LEAN, false>(P, actions, obs, reward, reward64, terminated, env, lane, ws, 0u, 0u, 0u, nullptr, 0, false);
+  } else {
+    if (obs16) fx_step_env<STRAT, REWARD, FAST5, true, LEAN>(P, actions, obs, reward, reward64, terminated, env, lane, ws, 0u, 0u, 0u, obs16, stride16);
+    else fx_step_env<STRAT, REWARD, FAST5, false, LEAN>(P, actions, obs, reward, reward64, terminated, env, lane, ws);
+  }
   if (sync.done_cnt) {  // this env's row (float32 and bf16) and state are complete: count it for its tile
     __syncwarp();
     if (lane == 0) {
@@ -1332,12 +1398,16 @@ fx_rollout_kernel(const __grid_constant__ FxKernelParams P, const char* __restri
 #if defined(FXENV_ENABLE_TIMING) || defined(FXENV_ENABLE_TIMELINE)
       if (P.timeline && lane == 0) { long long g__; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g__)); P.timeline[((size_t)k * N + env) * 2] = g__; }
 #endif
-      carry = fx_step_env<STRAT, REWARD, FAST5, false, LEAN, true, RESIDENT>(P, actions, obs, reward, nullptr, terminated, (int)env,
-                                                                           lane, ws, phase, k * N, slot_row, nullptr, 0, carry);
+      if constexpr (STRAT >= FX_KSTRAT_REPEAT)  // action repeat: the decision's substeps, one window copy among them
+        carry = fx_step_repeat<STRAT, REWARD, FAST5, false, LEAN, RESIDENT>(P, actions, obs, reward, nullptr, terminated, (int)env,
+                                                                          lane, ws, phase, k * N, slot_row, nullptr, 0, carry);
+      else
+        carry = fx_step_env<STRAT, REWARD, FAST5, false, LEAN, true, RESIDENT>(P, actions, obs, reward, nullptr, terminated, (int)env,
+                                                                             lane, ws, phase, k * N, slot_row, nullptr, 0, carry);
       slot_row += N;
       if (slot_row == (unsigned)obs_slots * N) slot_row = 0u;
       __syncwarp();
-      phase++;
+      phase++;  // every step (every decision, with the repeat) issued and waited on exactly one copy
 #if defined(FXENV_ENABLE_TIMING) || defined(FXENV_ENABLE_TIMELINE)
       if (P.timeline && lane == 0) { long long g__; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g__)); P.timeline[((size_t)k * N + env) * 2 + 1] = g__; }
 #endif
@@ -1453,27 +1523,44 @@ RolloutKernel pick_rollout_reward(int reward, int mode, bool resident) {
 
 int kernel_mode(const FxKernelParams& P, int lean) { return (lean && P.fast_features == 5) ? 2 : (P.fast_features == 5 ? 1 : 0); }
 
-// audit < 0: the variant for the current state of the bracket audit (P.audit)
-StepKernel pick_kernel(const FxKernelParams& P, int lean = -1, int audit = -1) {
+// The kernel template STRAT of a launch: the strategy, FX_KSTRAT_ATR_AUDIT for the ATR strategy while the bracket audit
+// is on, plus FX_KSTRAT_REPEAT while the action repeat is on.  audit / repeat < 0: the current state of the handle
+// (P.audit, P.repeat), else that variant.
+int kernel_strat(const FxKernelParams& P, int audit, int repeat) {
+  int s = P.cfg.strategy;
+  if (s == FX_STRATEGY_ATR_SLTP && (audit < 0 ? P.audit != nullptr : audit != 0)) s = FX_KSTRAT_ATR_AUDIT;
+  if (repeat < 0 ? P.repeat > 1 : repeat != 0) s += FX_KSTRAT_REPEAT;
+  return s;
+}
+
+StepKernel pick_kernel(const FxKernelParams& P, int lean = -1, int audit = -1, int repeat = -1) {
   const int mode = kernel_mode(P, lean < 0 ? P.lean : lean);
-  switch (P.cfg.strategy) {
-    case FX_STRATEGY_DEFAULT: return pick_reward<FX_STRATEGY_DEFAULT>(P.cfg.reward, mode);
-    case FX_STRATEGY_FIXED_SLTP: return pick_reward<FX_STRATEGY_FIXED_SLTP>(P.cfg.reward, mode);
-    default:
-      return (audit < 0 ? P.audit != nullptr : audit != 0) ? pick_reward<FX_KSTRAT_ATR_AUDIT>(P.cfg.reward, mode)
-                                                            : pick_reward<FX_STRATEGY_ATR_SLTP>(P.cfg.reward, mode);
+  const int r = P.cfg.reward;
+  switch (kernel_strat(P, audit, repeat)) {
+    case FX_STRATEGY_DEFAULT: return pick_reward<FX_STRATEGY_DEFAULT>(r, mode);
+    case FX_STRATEGY_FIXED_SLTP: return pick_reward<FX_STRATEGY_FIXED_SLTP>(r, mode);
+    case FX_STRATEGY_ATR_SLTP: return pick_reward<FX_STRATEGY_ATR_SLTP>(r, mode);
+    case FX_KSTRAT_ATR_AUDIT: return pick_reward<FX_KSTRAT_ATR_AUDIT>(r, mode);
+    case FX_KSTRAT_REPEAT + FX_STRATEGY_DEFAULT: return pick_reward<FX_KSTRAT_REPEAT + FX_STRATEGY_DEFAULT>(r, mode);
+    case FX_KSTRAT_REPEAT + FX_STRATEGY_FIXED_SLTP: return pick_reward<FX_KSTRAT_REPEAT + FX_STRATEGY_FIXED_SLTP>(r, mode);
+    case FX_KSTRAT_REPEAT + FX_STRATEGY_ATR_SLTP: return pick_reward<FX_KSTRAT_REPEAT + FX_STRATEGY_ATR_SLTP>(r, mode);
+    default: return pick_reward<FX_KSTRAT_REPEAT + FX_KSTRAT_ATR_AUDIT>(r, mode);
   }
 }
 
-RolloutKernel pick_rollout(const FxKernelParams& P, int lean = -1, int audit = -1) {
+RolloutKernel pick_rollout(const FxKernelParams& P, int lean = -1, int audit = -1, int repeat = -1) {
   const int mode = kernel_mode(P, lean < 0 ? P.lean : lean);
   const bool res = P.order_smem != 0;
-  switch (P.cfg.strategy) {
-    case FX_STRATEGY_DEFAULT: return pick_rollout_reward<FX_STRATEGY_DEFAULT>(P.cfg.reward, mode, res);
-    case FX_STRATEGY_FIXED_SLTP: return pick_rollout_reward<FX_STRATEGY_FIXED_SLTP>(P.cfg.reward, mode, res);
-    default:
-      return (audit < 0 ? P.audit != nullptr : audit != 0) ? pick_rollout_reward<FX_KSTRAT_ATR_AUDIT>(P.cfg.reward, mode, res)
-                                                            : pick_rollout_reward<FX_STRATEGY_ATR_SLTP>(P.cfg.reward, mode, res);
+  const int r = P.cfg.reward;
+  switch (kernel_strat(P, audit, repeat)) {
+    case FX_STRATEGY_DEFAULT: return pick_rollout_reward<FX_STRATEGY_DEFAULT>(r, mode, res);
+    case FX_STRATEGY_FIXED_SLTP: return pick_rollout_reward<FX_STRATEGY_FIXED_SLTP>(r, mode, res);
+    case FX_STRATEGY_ATR_SLTP: return pick_rollout_reward<FX_STRATEGY_ATR_SLTP>(r, mode, res);
+    case FX_KSTRAT_ATR_AUDIT: return pick_rollout_reward<FX_KSTRAT_ATR_AUDIT>(r, mode, res);
+    case FX_KSTRAT_REPEAT + FX_STRATEGY_DEFAULT: return pick_rollout_reward<FX_KSTRAT_REPEAT + FX_STRATEGY_DEFAULT>(r, mode, res);
+    case FX_KSTRAT_REPEAT + FX_STRATEGY_FIXED_SLTP: return pick_rollout_reward<FX_KSTRAT_REPEAT + FX_STRATEGY_FIXED_SLTP>(r, mode, res);
+    case FX_KSTRAT_REPEAT + FX_STRATEGY_ATR_SLTP: return pick_rollout_reward<FX_KSTRAT_REPEAT + FX_STRATEGY_ATR_SLTP>(r, mode, res);
+    default: return pick_rollout_reward<FX_KSTRAT_REPEAT + FX_KSTRAT_ATR_AUDIT>(r, mode, res);
   }
 }
 
@@ -1534,27 +1621,30 @@ cudaError_t fx_configure_kernels(FxKernelParams& P) {
   P.num_sms = sms > 0 ? sms : 1;
   P.resident_blocks = 0;
   // both the general and the LEAN instantiation: which one runs is only known once the candle tables are loaded; for
-  // the ATR strategy also both states of the bracket audit
-  const int n_lean = P.fast_features == 5 ? 2 : 1;
-  for (int v = 0; v < n_lean * (P.cfg.strategy == FX_STRATEGY_ATR_SLTP ? 2 : 1); v++) {
-    const int lean = v % n_lean, audit = v / n_lean;
-    cudaError_t e = cudaFuncSetAttribute(pick_kernel(P, lean, audit), cudaFuncAttributePreferredSharedMemoryCarveout, pct);
+  // the ATR strategy also both states of the bracket audit; and both states of the action repeat
+  const int n_lean = P.fast_features == 5 ? 2 : 1, n_audit = P.cfg.strategy == FX_STRATEGY_ATR_SLTP ? 2 : 1;
+  for (int v = 0; v < n_lean * n_audit * 2; v++) {
+    const int lean = v % n_lean, audit = (v / n_lean) % n_audit, repeat = v / (n_lean * n_audit);
+    const StepKernel sk = pick_kernel(P, lean, audit, repeat);
+    const RolloutKernel rk = pick_rollout(P, lean, audit, repeat);
+    cudaError_t e = cudaFuncSetAttribute(sk, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
     if (e != cudaSuccess) return e;
-    e = cudaFuncSetAttribute(pick_rollout(P, lean, audit), cudaFuncAttributePreferredSharedMemoryCarveout, rpct);
+    e = cudaFuncSetAttribute(rk, cudaFuncAttributePreferredSharedMemoryCarveout, rpct);
     if (e != cudaSuccess) return e;
     if (smem > 48 * 1024) {
-      e = cudaFuncSetAttribute(pick_kernel(P, lean, audit), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      e = cudaFuncSetAttribute(sk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return e;
     }
     if (rsmem > 48 * 1024) {
-      e = cudaFuncSetAttribute(pick_rollout(P, lean, audit), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rsmem);
+      e = cudaFuncSetAttribute(rk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rsmem);
       if (e != cudaSuccess) return e;
     }
     // how many CTAs of the persistent rollout kernel the device holds at once (= its grid size).  The minimum over every
-    // variant configured here, the bracket audit's included: one grid size serves whichever variant a launch picks, so a
-    // change that raises the audit kernels' registers or shared memory shrinks the grid with the log off as well
+    // variant configured here, the bracket audit's and the action repeat's included: one grid size serves whichever
+    // variant a launch picks, so a change that raises those kernels' registers or shared memory shrinks the grid with
+    // them off as well
     int per_sm = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pick_rollout(P, lean, audit), rcta * 32, rsmem);
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rk, rcta * 32, rsmem);
     if (e != cudaSuccess) return e;
     if (P.resident_blocks == 0 || sms * per_sm < P.resident_blocks) P.resident_blocks = sms * per_sm;
   }
@@ -1607,15 +1697,18 @@ int fx_rollout_warps(const FxKernelParams& P) { return fx_rollout_blocks(P) * ro
 // (N - warps) tickets ago, so nobody waits.  (Rounds that shrink towards the end of the batch -- "guided" scheduling, to
 // shorten the tail in which warps run dry -- cost more in extra hand-overs than they save in the tail.)  When every env has a warp of its own the whole batch is
 // one round: no hand-over at all.  FXENV_CHUNK=c forces chunks of c steps (measurements, tests).
+// With the action repeat (P.repeat = k > 1) a step spans up to k bars: the 64-step bound becomes a bound of 64 bars,
+// max(1, 64 / k) decisions, so that a ticket -- and the batch's tail -- is no longer than without the repeat.
 FxChunkPlan fx_rollout_plan(const FxKernelParams& P, int n_steps) {
   const char* fe = getenv("FXENV_CHUNK");  // read per launch: tests switch it between batches
   const int forced = fe ? atoi(fe) : 0;
   const long long warps = fx_rollout_warps(P);
   const long long N = P.cfg.num_envs;
+  const int max_chunk = P.repeat > 1 ? (64 / P.repeat > 1 ? 64 / P.repeat : 1) : 64;
   int chunk;
   if (forced > 0) chunk = forced;
   else if (N <= warps) chunk = n_steps;
-  else { chunk = (int)((N * (long long)n_steps) / (warps * 6)); if (chunk > 64) chunk = 64; }
+  else { chunk = (int)((N * (long long)n_steps) / (warps * 6)); if (chunk > max_chunk) chunk = max_chunk; }
   if (chunk < 1) chunk = 1;
   if (chunk > n_steps) chunk = n_steps;
   FxChunkPlan pl = {};

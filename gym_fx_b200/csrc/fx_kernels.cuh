@@ -82,6 +82,10 @@ struct FxKernelParams {
   double* audit;
   int64_t* audit_written;
   int32_t audit_cap;
+  // action repeat (fxenv_set_action_repeat): substeps per step (1 = off: the kernels without repeat run) and the
+  // FXENV_REPEAT_* flags.  A setting of the handle, not env state: outside the slab, like the audit.
+  int32_t repeat;
+  uint32_t repeat_flags;
 };
 
 // warps (= envs) per CTA of the step kernel.  One warp per CTA lets the second wave back-fill SM slots as soon as a

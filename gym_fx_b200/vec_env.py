@@ -64,6 +64,7 @@ class VecFxEnv:
         self.action_dtype = torch.float32 if cfg.action_mode == 1 else torch.int32
         self._policies: list = []
         self._audit = None  # (ring [N, capacity, 8], written [N], read cursor [N]) while the bracket audit is on
+        self.action_repeat = (1, False)  # (k, hold): set_action_repeat
 
     # ------------------------------------------------------------------ lifecycle
     def close(self):
@@ -107,6 +108,7 @@ class VecFxEnv:
 
     def step(self, actions: torch.Tensor, out_obs: Optional[torch.Tensor] = None):
         """-> (obs, reward float32 [N], terminated bool [N], truncated bool [N], info).
+        One step is one decision: with an action repeat k > 1 (set_action_repeat) it runs up to k bars.
         The returned tensors are views of buffers that the next step() overwrites."""
         a = actions
         if a.dtype != self.action_dtype or a.device != self.device or not a.is_contiguous():
@@ -155,7 +157,7 @@ class VecFxEnv:
 
     def step_many(self, actions: torch.Tensor, obs_ring: torch.Tensor, rewards: torch.Tensor, terminated: torch.Tensor):
         """K consecutive steps with all actions supplied up front (replay / random / scripted drivers); identical results
-        to K calls of step().  actions [K, N] (int32, or float32 in continuous mode); obs_ring float32 [slots, N, D]
+        to K calls of step().  A step is a decision (up to k bars with set_action_repeat).  actions [K, N] (int32, or float32 in continuous mode); obs_ring float32 [slots, N, D]
         (step k writes slot k % slots); rewards float32 [K, N]; terminated uint8 [K, N].  The library runs the batch as one
         persistent launch or as a cached CUDA graph of single steps (`step_many_engine`)."""
         K = self._check_batch(actions, obs_ring, rewards, terminated)
@@ -184,7 +186,8 @@ class VecFxEnv:
 
     def step_host(self, actions_host: torch.Tensor, obs_host: torch.Tensor, reward_host: torch.Tensor,
                   terminated_host: torch.Tensor):
-        """Reference-facing call with (pinned) HOST tensors: H2D actions, one step, D2H results, synchronous."""
+        """Reference-facing call with (pinned) HOST tensors: H2D actions, one step (one decision: up to k bars with
+        set_action_repeat), D2H results, synchronous."""
         N, D = self.num_envs, self.obs_dim
         self._check("actions_host", actions_host, self.action_dtype, (N,), host=True)
         self._check("obs_host", obs_host, torch.float32, (N, D), host=True)
@@ -410,6 +413,25 @@ class VecFxEnv:
         out["dropped"] = dropped
         return out
 
+    # ------------------------------------------------------------------ action repeat
+    def set_action_repeat(self, k: int, hold: bool = False):
+        """One decision per k bars (1 <= k <= 256; 1 = off, the default): every later step(), step_many() decision,
+        step_host() and rollout() decision runs up to k bars.  hold=False applies the action on each of the k bars
+        (frame skip); hold=True applies it on the first bar only and holds (action 0) on the others.  A step stops early
+        at a bar that terminates the episode, and a terminated env's step is its auto-reset step alone.  The observation
+        is that after the step's last bar, the reward the float64 sum of the bars' rewards (include/fxenv.h
+        fxenv_set_action_repeat).  A setting of the handle, not of the env state: snapshots and reset() keep it."""
+        if isinstance(k, bool) or int(k) != k:
+            raise ValueError(f"action repeat must be an integer, got {k!r}")
+        k = int(k)
+        if not 1 <= k <= _native.MAX_REPEAT:
+            raise ValueError(f"action repeat must be in [1, {_native.MAX_REPEAT}], got {k}")
+        rc = self.L.fxenv_set_action_repeat(self._h, k, _native.REPEAT_HOLD if hold else 0)
+        if rc == -1:
+            raise ValueError(self.L.fxenv_last_error(self._h).decode())
+        _native.check(self.L, self._h, rc, "fxenv_set_action_repeat")
+        self.action_repeat = (k, bool(hold))
+
     # ------------------------------------------------------------------ closed loop (policy on the device)
     def make_policy(self, weights=None) -> "FusedPolicy":
         """An actor-critic MLP(obs_dim, 256, 256) evaluated by the fused tensor-core kernel (fxenv.h: FxPolicy)."""
@@ -419,7 +441,8 @@ class VecFxEnv:
                 gumbel: Optional[torch.Tensor] = None, seed: int = 0, noise: Optional[torch.Tensor] = None,
                 deterministic: bool = False) -> Dict[str, torch.Tensor]:
         """`horizon` closed-loop steps (policy -> sample -> env.step) from the current state, all on the device: the
-        loop of the reference's driver (app/main.py:57-65) with a learned policy.  Returns / fills `buffers`:
+        loop of the reference's driver (app/main.py:57-65) with a learned policy.  A step is one policy decision: with an
+        action repeat k > 1 (set_action_repeat) the env runs up to k bars between two evaluations.  Returns / fills `buffers`:
         obs [H+1, N, D] (obs[t] is what the policy saw at step t), actions [H, N] (int32, or float32 in continuous mode),
         logp [H, N], value [H+1, N] (value[H] bootstraps), reward [H, N], done uint8 [H, N].
         Sampling noise for reproducible rollouts -- discrete mode: gumbel, float32 [H, N, 3] Gumbel(0,1); continuous

@@ -20,6 +20,7 @@
  *   fxenv_get_state/set_state      (no counterpart: env snapshot, SURVEY 8f #4)
  *   fxenv_rollout / fxenv_rollout_ex  the caller loop of app/main.py:57-65 with a learned policy (see below);
  *                                  continuous actions are the Box(-1, 1, (1,)) of app/env.py:71-80, 187-204
+ *   fxenv_set_action_repeat        (no counterpart: k bars per step, one decision per step; its contract below)
  *
  * Conventions: every function returns 0 on success, <0 on error (see FXENV_E_*); fxenv_last_error() gives the
  * message.  No exceptions or aborts cross the ABI.  The library owns env state (device struct-of-arrays) behind
@@ -318,6 +319,36 @@ typedef struct FxAuditPtrs {
 } FxAuditPtrs;
 
 int fxenv_get_bracket_audit(FxEnv* env, FxAuditPtrs* out);
+
+/* ---- action repeat: one step spans up to k bars, with one observation and one decision per step (no reference
+ * counterpart: the frame_skip of vectorised RL envs; "act every k bars") --------------------------------------------
+ * A handle has an action repeat k (1 <= k <= FXENV_MAX_REPEAT, default 1) and a mode:
+ *   repeat (flags 0, the default): the step's action is applied on each of the k bars (Atari frame-skip);
+ *   hold (FXENV_REPEAT_HOLD): the action is applied on the first bar only; the other bars run with the hold action --
+ *     the coerced action 0 itself, not a raw action that is thresholded.
+ * One step of fxenv_step / fxenv_step_host, and one decision of fxenv_step_many and fxenv_rollout, consists of up to k
+ * SUBSTEPS, each exactly one step of the library without repeat (so parity with the reference covers each of them):
+ *   1. An env that is terminated when the step begins runs one substep only: what a step does today (the auto-reset
+ *      step: reward 0, not done, observation of the new episode; without auto-reset (obs, 0.0, True)).  Substeps never
+ *      continue into a new episode.
+ *   2. Otherwise substeps j = 0, 1, ... run in order; the step stops after substep k - 1 or after the first substep that
+ *      terminates (broke, or data exhausted).  "The first step does not advance the bar" holds per substep: the first
+ *      decision of an episode covers k - 1 new bars, as the expanded action stream does in the reference.
+ *   3. The observation is that of the state after the last substep run, `terminated` is that substep's flag, and the
+ *      reward is the float64 sum of the substep rewards in substep order, starting from r0 (so k = 1 keeps the sign of
+ *      a zero): reward64 is that sum, reward (float) of it.  With the Sharpe reward this is a sum of k rolling Sharpe
+ *      values.
+ *   4. All state advances per substep: account, order table, run statistics, Sharpe deque, drawdown peak, running
+ *      z-score statistics, episode records and the bracket audit (one record per bar that logs, with that bar's row).
+ *      The info columns after a step are those after its last substep.
+ * Equivalently: for every env, the outputs of a step equal those of the library without repeat driven by the env's
+ * expanded action stream, taken at the step's last substep, with the rewards summed as above.
+ * k and the mode belong to the handle, like the bracket audit, and are not env state: fxenv_state_bytes, snapshots,
+ * fxenv_reset and fxenv_set_state neither include nor change them.  Changing them drops the cached step-many graphs and
+ * makes each policy re-capture its rollout graph.  Out-of-range repeat or unknown flag bits: FXENV_E_INVALID. */
+#define FXENV_MAX_REPEAT 256
+#define FXENV_REPEAT_HOLD 1u
+int fxenv_set_action_repeat(FxEnv* env, int32_t repeat, uint32_t flags);
 
 /* ---- closed loop: a policy on the device between the steps ------------------------------------------------------
  * Replaces the caller loop of app/main.py:57-65 (`action = strategy.decide_action(obs, info, step); env.step(action)`)
