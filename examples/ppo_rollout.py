@@ -3,7 +3,7 @@
 examples/ppo_rollout.py -- PPO on the device-resident env (SURVEY section 8(f) rank 1; BASELINE configs[3] shape).
 
 One process per GPU.  Each rank owns a shard of envs (gym_fx_b200.VecFxEnv, no collective in the step path) and a
-replica of an actor-critic MLP(256, 256).  A rollout of H steps runs entirely on the device: the fused wgmma policy
+replica of an actor-critic MLP(hidden, hidden) (--hidden 64, 128, 256 or 512; default 256).  A rollout of H steps runs entirely on the device: the fused wgmma policy
 kernel and the env step kernel alternate (VecFxEnv.rollout -> fxenv_rollout, a cached CUDA graph of 2H + 2 kernels), the
 observations never leave the GPU.  The PPO update is plain torch; gradients are averaged by ONE flat NCCL all-reduce per
 minibatch and advantages are normalised with global statistics (gym_fx_b200.learner / gym_fx_b200.sharding).
@@ -12,6 +12,7 @@ minibatch and advantages are normalised with global statistics (gym_fx_b200.lear
     python examples/ppo_rollout.py --envs 4096 --action-space continuous --updates 5 --eval-rollouts 2
     python examples/ppo_rollout.py --envs 4096 --episode-bars 500 --holdout-frac 0.2 --eval-rollouts 2
     python examples/ppo_rollout.py --envs 4096 --action-repeat 5 --repeat-mode hold
+    python examples/ppo_rollout.py --hidden 64
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 examples/ppo_rollout.py --envs 4096
 
 --action-space continuous trains a Gaussian actor on the Box(-1, 1) action (thresholded to hold / long / short by the
@@ -59,6 +60,8 @@ def main():
     ap.add_argument("--action-repeat", type=int, default=1, help="bars per decision (1..256)")
     ap.add_argument("--repeat-mode", choices=("repeat", "hold"), default="repeat",
                     help="repeat: the action on every bar of a step; hold: on its first bar, then hold")
+    ap.add_argument("--hidden", type=int, choices=(64, 128, 256, 512), default=256,
+                    help="width of both hidden layers of the actor-critic")
     args = ap.parse_args()
     continuous = args.action_space == "continuous"
     if not 0.0 <= args.holdout_frac < 1.0:
@@ -109,7 +112,7 @@ def main():
 
     torch.backends.cuda.matmul.allow_tf32 = True
     torch.manual_seed(0)  # identical replicas on every rank
-    net = ActorCritic(D, continuous=continuous).to(dev)
+    net = ActorCritic(D, hidden=args.hidden, continuous=continuous).to(dev)
     opt = torch.optim.Adam(net.parameters(), lr=args.lr, eps=1e-5)
     policy = env.make_policy(net)
     buf = None
@@ -175,9 +178,9 @@ def main():
         steps = N * world * H * n_it
         print(json.dumps({
             "example": "ppo_rollout", "workload": desc, "n_gpus": world, "envs_per_gpu": N, "horizon": H,
-            "policy": f"MLP({D},256,256) actor-critic ({args.action_space} actions), fused wgmma kernel in the rollout, "
+            "policy": f"MLP({D},{args.hidden},{args.hidden}) actor-critic ({args.action_space} actions), fused wgmma kernel in the rollout, "
                       "torch (tf32) in the update",
-            "rollout_env_steps_per_s": steps / max(t_roll, 1e-9), "rollout_us_per_step": t_roll / (H * n_it) * 1e6,
+            "hidden": args.hidden, "rollout_env_steps_per_s": steps / max(t_roll, 1e-9), "rollout_us_per_step": t_roll / (H * n_it) * 1e6,
             "action_repeat": K, "repeat_mode": args.repeat_mode,
             "rollout_bars_per_s_upper_bound": steps * K / max(t_roll, 1e-9),
             "train_env_steps_per_s": steps / max(t_roll + t_upd, 1e-9), "update_s": t_upd / n_it, **stats}), flush=True)

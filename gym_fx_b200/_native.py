@@ -31,12 +31,13 @@ EXPORTS = [
     "fxenv_state_bytes", "fxenv_get_state", "fxenv_set_state", "fxenv_launch_count", "fxenv_step_many_engine",
     "fxenv_policy_create", "fxenv_policy_set_weights", "fxenv_policy_destroy", "fxenv_rollout", "fxenv_policy_sync_timeouts",
     "fxenv_rollout_ex", "fxenv_policy_peek", "fxenv_set_reset_starts", "fxenv_get_episode_info",
-    "fxenv_set_bracket_audit", "fxenv_get_bracket_audit", "fxenv_set_action_repeat",
+    "fxenv_set_bracket_audit", "fxenv_get_bracket_audit", "fxenv_set_action_repeat", "fxenv_policy_create_ex",
 ]
 
 ROLLOUT_GREEDY = 1  # FXENV_ROLLOUT_GREEDY
 PEEK_OBS16, PEEK_H1 = 0, 1  # FXENV_PEEK_*
 MAX_REPEAT, REPEAT_HOLD = 256, 1  # FXENV_MAX_REPEAT, FXENV_REPEAT_HOLD
+POLICY_WIDTHS = (64, 128, 256, 512)  # the hidden widths fxenv_policy_create_ex accepts
 
 
 class FxEnvError(RuntimeError):
@@ -130,6 +131,7 @@ def load():
     L.fxenv_step_many_engine.restype = C.c_int
     L.fxenv_step_many_engine.argtypes = [vp, C.c_int]
     L.fxenv_policy_create.argtypes = [vp, C.POINTER(vp)]
+    L.fxenv_policy_create_ex.argtypes = [vp, C.c_int32, C.POINTER(vp)]
     L.fxenv_policy_set_weights.argtypes = [vp, C.POINTER(FxPolicyWeights), vp]
     L.fxenv_policy_destroy.argtypes = [vp]
     L.fxenv_rollout.argtypes = [vp, vp, C.POINTER(FxRollout), vp]

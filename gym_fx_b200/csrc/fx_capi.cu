@@ -706,11 +706,12 @@ int fxenv_debug_timings(FxEnv* env, long long* out_host) {
 struct FxPolicy {
   FxEnv* env = nullptr;
   int k_pad = 0;                       // obs_dim padded to a multiple of 64 (bf16 row stride of the observation copy)
-  uint16_t* w1 = nullptr;              // bf16 [256][k_pad]
-  uint16_t* w2 = nullptr;              // bf16 [256][256]
-  float* fparams = nullptr;            // b1[256] | b2[256] | head_w[4][256] | head_b[4]
+  int hidden = FX_POLICY_HIDDEN;       // width of both hidden layers: 64, 128, 256 or 512 (fxenv_policy_create_ex)
+  uint16_t* w1 = nullptr;              // bf16 [hidden][k_pad]
+  uint16_t* w2 = nullptr;              // bf16 [hidden][hidden]
+  float* fparams = nullptr;            // b1[hidden] | b2[hidden] | head_w[4][hidden] | head_b[4]
   uint16_t* obs16[2] = {nullptr, nullptr};  // bf16 [num_envs][k_pad], double buffered
-  uint16_t* h1 = nullptr;              // bf16 [num_envs padded to whole tiles][256]: the two halves of h1 meet here
+  uint16_t* h1 = nullptr;              // bf16 [num_envs padded to whole tiles][hidden]: the two halves of h1 meet here
   float* head_part = nullptr;          // float4 [num_envs padded]: partial head sums of the second CTA of a pair
   int32_t* sync = nullptr;             // act_flag[tiles] | done_cnt[tiles] | timeouts[1] (FxTileSync), zeroed per rollout
   int tiles = 0;
@@ -795,7 +796,7 @@ cudaError_t enqueue_rollout(FxEnv* env, FxPolicy* pol, const FxRollout& io, uint
     for (int t = 0; t <= H; t++) {
       const bool last = (t == H);  // the bootstrap evaluation: value only
       if (!(skip & 2))
-      e = fx_launch_policy(pol->map_obs[t & 1], pol->map_w1, pol->map_w2, pol->map_h1, pol->dev, (int)N, pol->k_pad,
+      e = fx_launch_policy(pol->map_obs[t & 1], pol->map_w1, pol->map_w2, pol->map_h1, pol->dev, pol->hidden, (int)N, pol->k_pad,
                            (!last && io.gumbel) ? io.gumbel + (size_t)t * N * noise_per_env : nullptr, io.seed, (unsigned)t,
                            last ? static_cast<void*>(pol->scratch_act) : actions + (size_t)t * N,
                            last ? pol->scratch_logp : io.logp + (size_t)t * N, io.value + (size_t)t * N, sg, (int)e0, (int)e1,
@@ -857,7 +858,7 @@ int64_t fxenv_policy_peek(FxPolicy* pol, int what, int slot, void* dst, int64_t 
     n = (int64_t)env->P.cfg.num_envs * pol->k_pad * 2;
   } else if (what == FXENV_PEEK_H1 && slot == 0) {
     src = pol->h1;
-    n = (int64_t)pol->tiles * FX_POLICY_TILE_M * FX_POLICY_HIDDEN * 2;
+    n = (int64_t)pol->tiles * FX_POLICY_TILE_M * pol->hidden * 2;
   } else {
     return fail(env, FXENV_E_INVALID, "fxenv_policy_peek: unknown buffer or slot");
   }
@@ -869,18 +870,25 @@ int64_t fxenv_policy_peek(FxPolicy* pol, int what, int slot, void* dst, int64_t 
 }
 
 int fxenv_policy_create(FxEnv* env, FxPolicy** out) {
+  return fxenv_policy_create_ex(env, FX_POLICY_HIDDEN, out);
+}
+
+int fxenv_policy_create_ex(FxEnv* env, int32_t hidden, FxPolicy** out) {
   if (!env || !out) return FXENV_E_INVALID;
   *out = nullptr;
   if (env->P.cfg.action_mode != FX_ACTION_DISCRETE && env->P.cfg.action_mode != FX_ACTION_CONTINUOUS)
     return fail(env, FXENV_E_INVALID, "unknown action mode");
+  if (!fx_policy_width_ok(hidden))
+    return fail(env, FXENV_E_INVALID, "policy width must be 64, 128, 256 or 512, got " + std::to_string(hidden));
   DeviceGuard g(env->device);
   FxPolicy* pol = new (std::nothrow) FxPolicy();
   if (!pol) return fail(env, FXENV_E_NOMEM, "out of host memory");
   pol->env = env;
   pol->continuous = env->P.cfg.action_mode == FX_ACTION_CONTINUOUS;
+  pol->hidden = hidden;
   const size_t N = (size_t)env->P.cfg.num_envs, D = (size_t)env->P.obs_dim;
   pol->k_pad = (int)((D + 63) / 64 * 64);
-  const size_t KP = (size_t)pol->k_pad, Hd = FX_POLICY_HIDDEN;
+  const size_t KP = (size_t)pol->k_pad, Hd = (size_t)hidden;
   bool ok = cudaMalloc(&pol->w1, Hd * KP * 2) == cudaSuccess && cudaMalloc(&pol->w2, Hd * Hd * 2) == cudaSuccess &&
             cudaMalloc(&pol->fparams, (2 * Hd + 4 * Hd + 4) * sizeof(float)) == cudaSuccess &&
             cudaMalloc(&pol->obs16[0], N * KP * 2) == cudaSuccess && cudaMalloc(&pol->obs16[1], N * KP * 2) == cudaSuccess &&
@@ -901,8 +909,8 @@ int fxenv_policy_create(FxEnv* env, FxPolicy** out) {
   cudaMemset(pol->sync, 0, (2 * (size_t)pol->tiles + 1) * sizeof(int32_t));
   int rc = make_map(env, &pol->map_obs[0], pol->obs16[0], N, KP, FX_POLICY_TILE_M);
   if (!rc) rc = make_map(env, &pol->map_obs[1], pol->obs16[1], N, KP, FX_POLICY_TILE_M);
-  if (!rc) rc = make_map(env, &pol->map_w1, pol->w1, Hd, KP, FX_POLICY_HIDDEN / 2);   // a CTA loads its half of the units
-  if (!rc) rc = make_map(env, &pol->map_w2, pol->w2, Hd, Hd, FX_POLICY_HIDDEN / 2);
+  if (!rc) rc = make_map(env, &pol->map_w1, pol->w1, Hd, KP, (uint32_t)Hd / 2);   // a CTA loads its half of the units
+  if (!rc) rc = make_map(env, &pol->map_w2, pol->w2, Hd, Hd, (uint32_t)Hd / 2);
   if (!rc) rc = make_map(env, &pol->map_h1, pol->h1, NP, Hd, FX_POLICY_TILE_M);
   if (rc) { fxenv_policy_destroy(pol); return rc; }
   cudaError_t ce = fx_policy_configure();
@@ -920,7 +928,7 @@ int fxenv_policy_set_weights(FxPolicy* pol, const FxPolicyWeights* w, void* stre
   if (!w->w1 || !w->b1 || !w->w2 || !w->b2 || !w->w_pi || !w->b_pi || !w->w_v || !w->b_v) return fail(env, FXENV_E_INVALID, "null weight pointer");
   DeviceGuard g(env->device);
   cudaStream_t s = (cudaStream_t)stream_;
-  const int D = env->P.obs_dim, Hd = FX_POLICY_HIDDEN;
+  const int D = env->P.obs_dim, Hd = pol->hidden;
   FX_CUDA(env, fx_policy_pack(w->w1, pol->w1, Hd, D, pol->k_pad, s));
   FX_CUDA(env, fx_policy_pack(w->w2, pol->w2, Hd, Hd, Hd, s));
   float* f = pol->fparams;

@@ -1,6 +1,6 @@
 """
-PPO learner glue for the closed loop (BASELINE configs[3]: PPO MLP(256,256) actor-critic on sharpe_reward envs, NCCL
-gradient all-reduce).  This is CALLER code of the hot path -- the counterpart of the loop in app/main.py:57-65 for a
+PPO learner glue for the closed loop (BASELINE configs[3]: PPO actor-critic on sharpe_reward envs, NCCL gradient
+all-reduce; the MLP is 256 x 256 by default, and the fused loop also runs widths 64, 128 and 512: ActorCritic(hidden=...)).  This is CALLER code of the hot path -- the counterpart of the loop in app/main.py:57-65 for a
 learned policy -- written in plain torch (autograd for the backward pass):
 
     rollout   VecFxEnv.rollout: fused wgmma policy kernel <-> env step kernel, H steps, nothing leaves the device

@@ -433,9 +433,10 @@ class VecFxEnv:
         self.action_repeat = (k, bool(hold))
 
     # ------------------------------------------------------------------ closed loop (policy on the device)
-    def make_policy(self, weights=None) -> "FusedPolicy":
-        """An actor-critic MLP(obs_dim, 256, 256) evaluated by the fused tensor-core kernel (fxenv.h: FxPolicy)."""
-        return FusedPolicy(self, weights)
+    def make_policy(self, weights=None, hidden: Optional[int] = None) -> "FusedPolicy":
+        """An actor-critic MLP(obs_dim, hidden, hidden) evaluated by the fused tensor-core kernel (fxenv.h: FxPolicy).
+        hidden: 64, 128, 256 or 512; None takes it from the weights (the rows of w1), or 256 without weights."""
+        return FusedPolicy(self, weights, hidden)
 
     def rollout(self, policy: "FusedPolicy", horizon: int, buffers: Optional[Dict[str, torch.Tensor]] = None,
                 gumbel: Optional[torch.Tensor] = None, seed: int = 0, noise: Optional[torch.Tensor] = None,
@@ -537,24 +538,42 @@ def _tensor_from_ptr(ptr: int, n: int, dtype: torch.dtype, device: torch.device)
 
 
 class FusedPolicy:
-    """Device-resident actor-critic MLP(obs_dim, 256, 256) -> 3 logits + value, evaluated between env steps by the fused
-    wgmma kernel (gym_fx_b200/csrc/fx_policy.cu).  `set_weights` takes float32 CUDA tensors in torch.nn.Linear layout
-    (or a module with .body[0], .body[2], .pi, .v like gym_fx_b200.learner.ActorCritic).
-    In continuous action mode the actor is a Gaussian: `pi` is Linear(256, 1) (the mean) and a `log_std` tensor of shape
-    [1] (dict key "log_std", or the module's .log_std parameter) gives the state-independent log sigma."""
+    """Device-resident actor-critic MLP(obs_dim, hidden, hidden) -> 3 logits + value, evaluated between env steps by the
+    fused wgmma kernel (gym_fx_b200/csrc/fx_policy.cu).  `set_weights` takes float32 CUDA tensors in torch.nn.Linear
+    layout (or a module with .body[0], .body[2], .pi, .v like gym_fx_b200.learner.ActorCritic).
+    In continuous action mode the actor is a Gaussian: `pi` is Linear(hidden, 1) (the mean) and a `log_std` tensor of
+    shape [1] (dict key "log_std", or the module's .log_std parameter) gives the state-independent log sigma.
+    hidden (both layers): 64, 128, 256 or 512.  None takes the width from `weights` (module.body[0].out_features, or the
+    rows of weights["w1"]), or HIDDEN = 256 without weights; an explicit width that disagrees with the weights is a
+    ValueError.  The width is fixed for the life of the policy (`self.hidden`)."""
 
     HIDDEN = 256
 
-    def __init__(self, env: VecFxEnv, weights=None):
+    def __init__(self, env: VecFxEnv, weights=None, hidden: Optional[int] = None):
+        inferred = None if weights is None else self._width_of(weights)
+        if hidden is None:
+            hidden = self.HIDDEN if inferred is None else inferred
+        elif inferred is not None and int(hidden) != inferred:
+            raise ValueError(f"hidden={hidden} disagrees with the weights, which are {inferred} wide")
+        if int(hidden) not in _native.POLICY_WIDTHS:
+            raise ValueError(f"policy width must be one of {_native.POLICY_WIDTHS}, got {hidden}")
         self.env = env
+        self.hidden = int(hidden)
         self.continuous = env.action_dtype == torch.float32
         self._p = C.c_void_p()
-        rc = env.L.fxenv_policy_create(env._h, C.byref(self._p))
-        _native.check(env.L, env._h, rc, "fxenv_policy_create")
+        rc = env.L.fxenv_policy_create_ex(env._h, self.hidden, C.byref(self._p))
+        _native.check(env.L, env._h, rc, "fxenv_policy_create_ex")
         self._keep = None
         env._policies.append(self)
         if weights is not None:
             self.set_weights(weights)
+
+    @staticmethod
+    def _width_of(weights) -> int:
+        """hidden width of an ActorCritic-like module or a weight dict (the rows of w1)"""
+        if isinstance(weights, dict):
+            return int(weights["w1"].shape[0])
+        return int(weights.body[0].out_features)
 
     def sync_timeouts(self) -> int:
         """Polls of the last rollout's tile hand-over that gave up (0 unless something is broken); synchronises."""
@@ -566,7 +585,7 @@ class FusedPolicy:
     def peek(self, what: str, slot: int = 0) -> torch.Tensor:
         """Copy of an internal device buffer of the policy, for tests and debugging (fxenv_policy_peek), ordered on the
         current stream.  what = "obs16": the bf16 observation copy of `slot` (0 or 1) that the kernel reads,
-        [num_envs, k_pad]; "h1": the layer-1 activations of the last evaluation, [num_envs rounded up to 128, 256]."""
+        [num_envs, k_pad]; "h1": the layer-1 activations of the last evaluation, [num_envs rounded up to 128, hidden]."""
         code = {"obs16": _native.PEEK_OBS16, "h1": _native.PEEK_H1}.get(what)
         if code is None:
             raise ValueError(f"what must be 'obs16' or 'h1', got {what!r}")
@@ -574,7 +593,7 @@ class FusedPolicy:
         n = int(L.fxenv_policy_peek(self._p, code, int(slot), None, 0, s))
         if n < 0:
             _native.check(L, self.env._h, n, "fxenv_policy_peek")
-        cols = self.HIDDEN if what == "h1" else (self.env.obs_dim + 63) // 64 * 64
+        cols = self.hidden if what == "h1" else (self.env.obs_dim + 63) // 64 * 64
         out = torch.empty((n // (2 * cols), cols), dtype=torch.int16, device=self.env.device)
         rc = int(L.fxenv_policy_peek(self._p, code, int(slot), out.data_ptr(), n, s))
         if rc < 0:
@@ -590,7 +609,7 @@ class FusedPolicy:
                 if getattr(m, "log_std", None) is None:
                     raise ValueError("continuous action mode needs a log_std parameter of shape [1] on the module")
                 weights["log_std"] = m.log_std
-        D, Hd = self.env.obs_dim, self.HIDDEN
+        D, Hd = self.env.obs_dim, self.hidden
         n_pi = 1 if self.continuous else 3
         shapes = {"w1": (Hd, D), "b1": (Hd,), "w2": (Hd, Hd), "b2": (Hd,), "w_pi": (n_pi, Hd), "b_pi": (n_pi,), "w_v": (Hd,),
                   "b_v": (1,)}
@@ -605,7 +624,7 @@ class FusedPolicy:
                 t = t.reshape(-1)
             t = t.to(device=self.env.device, dtype=torch.float32).contiguous()
             if tuple(t.shape) != shape:
-                raise ValueError(f"{k} must have shape {shape}, got {tuple(t.shape)}")
+                raise ValueError(f"{k} must have shape {shape} for this {Hd}-wide policy, got {tuple(t.shape)}")
             ts[k] = t
         if self.continuous:  # FxPolicyWeights.b_pi in continuous mode: {b_mu, log sigma}
             ts["b_pi"] = torch.cat([ts["b_pi"], ts.pop("log_std")])

@@ -352,9 +352,10 @@ int fxenv_set_action_repeat(FxEnv* env, int32_t repeat, uint32_t flags);
 
 /* ---- closed loop: a policy on the device between the steps ------------------------------------------------------
  * Replaces the caller loop of app/main.py:57-65 (`action = strategy.decide_action(obs, info, step); env.step(action)`)
- * for a learned actor-critic (BASELINE configs[3]: PPO MLP(256,256)): observation rows never leave the GPU, and the
- * policy is one fused tensor-core kernel per step (wgmma / TMA / clusters, gym_fx_b200/csrc/fx_policy.cu), chained to the
- * env step kernel by programmatic dependent launches.  The actor head follows the env's FxConfig.action_mode:
+ * for a learned actor-critic MLP(hidden, hidden) (default 256, BASELINE configs[3]: PPO MLP(256,256)): observation rows
+ * never leave the GPU, and the policy is one fused tensor-core kernel per step (wgmma / TMA / clusters,
+ * gym_fx_b200/csrc/fx_policy.cu), chained to the env step kernel by programmatic dependent launches.  The actor head
+ * follows the env's FxConfig.action_mode:
  *
  *   h1 = tanh(obs W1^T + b1), h2 = tanh(h1 W2^T + b2), value = h2 wv + bv
  *   FX_ACTION_DISCRETE:   logits = h2 Wpi^T + bpi (3)
@@ -368,15 +369,16 @@ int fxenv_set_action_repeat(FxEnv* env, int32_t repeat, uint32_t flags);
  * this purpose); biases, heads, sampling and log-prob in float32. */
 typedef struct FxPolicy FxPolicy;
 
-/* DEVICE pointers to float32 parameters in torch.nn.Linear layout ([out][in] row-major). */
+/* DEVICE pointers to float32 parameters in torch.nn.Linear layout ([out][in] row-major); hidden = the policy's width
+ * (fxenv_policy_create_ex). */
 typedef struct FxPolicyWeights {
-  const float* w1;   /* [256][obs_dim] */
-  const float* b1;   /* [256] */
-  const float* w2;   /* [256][256] */
-  const float* b2;   /* [256] */
-  const float* w_pi; /* discrete: [3][256] (one row per action);  continuous: [1][256] (the mean) */
-  const float* b_pi; /* discrete: [3];                            continuous: [2] = {b_mu, log sigma} */
-  const float* w_v;  /* [256] */
+  const float* w1;   /* [hidden][obs_dim] */
+  const float* b1;   /* [hidden] */
+  const float* w2;   /* [hidden][hidden] */
+  const float* b2;   /* [hidden] */
+  const float* w_pi; /* discrete: [3][hidden] (one row per action);  continuous: [1][hidden] (the mean) */
+  const float* b_pi; /* discrete: [3];                               continuous: [2] = {b_mu, log sigma} */
+  const float* w_v;  /* [hidden] */
   const float* b_v;  /* [1] */
 } FxPolicyWeights;
 
@@ -401,8 +403,11 @@ typedef struct FxRollout {
 /* fxenv_rollout_ex flags */
 #define FXENV_ROLLOUT_GREEDY 1u   /* evaluation: the most likely action (argmax of the logits / the mean), no sampling */
 
-/* Discrete or continuous, as FxConfig.action_mode. */
+/* Discrete or continuous, as FxConfig.action_mode.  `hidden` is the width of both hidden layers: 64, 128, 256 or 512
+ * (anything else: FXENV_E_INVALID).  A 512-wide policy runs one kernel CTA per SM instead of two.
+ * fxenv_policy_create(env, out) is fxenv_policy_create_ex(env, 256, out). */
 int fxenv_policy_create(FxEnv* env, FxPolicy** out);
+int fxenv_policy_create_ex(FxEnv* env, int32_t hidden, FxPolicy** out);
 /* Converts / copies the parameters into the policy's own device buffers (stream-ordered; call after every optimiser step). */
 int fxenv_policy_set_weights(FxPolicy* pol, const FxPolicyWeights* weights_dev, void* stream);
 int fxenv_policy_destroy(FxPolicy* pol);
@@ -421,7 +426,7 @@ int fxenv_policy_sync_timeouts(FxPolicy* pol);
 #define FXENV_PEEK_OBS16 0   /* slot 0 | 1: the bf16 observation copy the policy reads, [num_envs][k_pad] (k_pad = obs_dim
                               * rounded up to a multiple of 64, zero pad columns); a rollout's step t reads slot t % 2 */
 #define FXENV_PEEK_H1 1      /* slot 0: the layer-1 activations of the last policy evaluation (after a rollout: the
-                              * bootstrap one), bf16 [num_envs rounded up to a multiple of 128][256] */
+                              * bootstrap one), bf16 [num_envs rounded up to a multiple of 128][hidden] */
 /* Test / debugging aid: stream-ordered copy of an internal policy buffer into caller DEVICE memory `dst` of `bytes`
  * bytes.  dst == NULL: returns the byte size needed.  Returns the bytes copied, or <0.  Reads only. */
 int64_t fxenv_policy_peek(FxPolicy* pol, int what, int slot, void* dst, int64_t bytes, void* stream);
