@@ -25,6 +25,13 @@ total return and maximum drawdown of each env's last finished episode (the reset
 evaluation, record the episodes they cut short).
 --action-repeat K lets the policy decide once per K bars (VecFxEnv.set_action_repeat): a rollout step is a decision,
 GAE runs per decision.  --repeat-mode repeat applies the action on every bar of the step, hold on its first bar only.
+--max-episode-steps M cuts every episode after M decisions and --truncate-window reports the end of an episode window
+(--episode-bars, or the table's end) as a cut instead of an end (VecFxEnv.set_time_limit): the rollout's done codes then
+tell truncations (2) from terminations (1), and GAE bootstraps through a truncation from the value of the cut episode's
+last observation instead of treating the cut as the end of the market.  Before training, the envs' episodes are
+staggered: in 8 groups, each reset after a different number of hold decisions, so that their cuts spread over the run
+instead of falling on the same step.  terminated_frac / truncated_frac: the share of the last rollout's steps with each
+code.
 Prints one JSON line: env-steps/s (decisions) of the rollout phase (policy in the loop) and of the whole train loop, and
 bars/s of the rollout phase as an upper bound (decisions x K: a step that ends an episode runs fewer bars).
 """
@@ -62,6 +69,10 @@ def main():
                     help="repeat: the action on every bar of a step; hold: on its first bar, then hold")
     ap.add_argument("--hidden", type=int, choices=(64, 128, 256, 512), default=256,
                     help="width of both hidden layers of the actor-critic")
+    ap.add_argument("--max-episode-steps", type=int, default=0,
+                    help="time limit: an episode is truncated after this many decisions (0: none)")
+    ap.add_argument("--truncate-window", action="store_true",
+                    help="the end of an episode window is a truncation (bootstrapped), not a termination")
     args = ap.parse_args()
     continuous = args.action_space == "continuous"
     if not 0.0 <= args.holdout_frac < 1.0:
@@ -70,6 +81,8 @@ def main():
         ap.error("--holdout-frac needs --episode-bars (an episode must fit inside its part of the table)")
     if not 1 <= args.action_repeat <= 256:
         ap.error("--action-repeat must be in 1..256")
+    if args.max_episode_steps < 0:
+        ap.error("--max-episode-steps must be >= 0")
 
     import bench
     from gym_fx_b200.learner import ActorCritic, ppo_update
@@ -99,7 +112,15 @@ def main():
     if K > 1:
         env.set_action_repeat(K, hold=args.repeat_mode == "hold")
         desc += f", one decision per {K} bars ({args.repeat_mode})"
+    if args.max_episode_steps > 0 or args.truncate_window:
+        env.set_time_limit(args.max_episode_steps, truncate_window=args.truncate_window)
+        if args.max_episode_steps > 0:
+            desc += f", episodes truncated after {args.max_episode_steps} decisions"
+        if args.truncate_window:
+            desc += ", window ends truncate"
     T, L = bench.T_BARS, args.episode_bars
+    truncating = args.max_episode_steps > 0 or args.truncate_window
+    stagger = (args.max_episode_steps if args.max_episode_steps > 0 else L) if truncating else 0   # decisions
     split = int(T * (1.0 - args.holdout_frac))       # training bars [0, split), held-out bars [split, T)
     if args.holdout_frac > 0.0:
         if split - L < 0 or T - L < split:
@@ -108,7 +129,19 @@ def main():
         env.set_episode_starts(0, split - L, seed=0x5EED0000 + rank)   # a window [start, start + L) inside training
         env.reset()
     else:
-        env.reset(torch.as_tensor(shard_starts(N, rank, world, T, (args.updates + args.eval_rollouts + 2) * H * K + 64, 256)))
+        env.reset(torch.as_tensor(shard_starts(N, rank, world, T, (args.updates + args.eval_rollouts + 2) * H * K + 64 + stagger * K,
+                                               256)))
+    if stagger > 0:   # group g restarts its episode after (g + 1) / 8 of the stagger: phases 0, 1/8, ... 7/8 of it
+        G, n = 8, max(1, stagger // 8)
+        hold = torch.zeros((n, N), dtype=env.action_dtype, device=dev)
+        ring = torch.empty((2, N, D), dtype=torch.float32, device=dev)
+        rews, codes = torch.empty((n, N), dtype=torch.float32, device=dev), torch.empty((n, N), dtype=torch.uint8, device=dev)
+        group = torch.arange(N, device=dev) % G
+        for g in range(G):
+            env.step_many(hold, ring, rews, codes)
+            env.reset(mask=group == g)
+        del ring, rews, codes
+    done_start = env.episode_stats()["episodes_done"].clone()   # the episodes the stagger cut short are not training's
 
     torch.backends.cuda.matmul.allow_tf32 = True
     torch.manual_seed(0)  # identical replicas on every rank
@@ -134,7 +167,9 @@ def main():
         if it > 0:                                        # the first iteration pays one-off set-up costs
             t_roll += t1 - t0
             t_upd += t2 - t1
-        stats.update(mean_reward=float(buf["reward"].mean()), terminated_frac=float(buf["done"].float().mean()))
+        d = buf["done"]   # 0 / 1, or the codes 1 = terminated, 2 = truncated with a time limit
+        stats.update(mean_reward=float(buf["reward"].mean()), terminated_frac=float((d == 1).float().mean()),
+                     truncated_frac=float((d == 2).float().mean()))
 
     def episode_report(prefix, done_before):
         """Episodes finished since `done_before` and the mean total return / max drawdown of each env's last finished one
@@ -153,7 +188,7 @@ def main():
     if holdout:   # every env into a fresh episode in the held-out tail; the reset records the training episodes it ends
         env.set_episode_starts(split, T - L, seed=0xE7A10000 + rank)
         env.reset()
-        stats.update(episode_report("train", torch.zeros_like(env.episode_stats()["episodes_done"])))
+        stats.update(episode_report("train", done_start))
         done0 = env.episode_stats()["episodes_done"].clone()
     if args.eval_rollouts > 0:   # greedy evaluation of the trained policy (held out: from the fresh episodes)
         rew_sum = torch.zeros((), dtype=torch.float64, device=dev)

@@ -32,12 +32,15 @@ EXPORTS = [
     "fxenv_policy_create", "fxenv_policy_set_weights", "fxenv_policy_destroy", "fxenv_rollout", "fxenv_policy_sync_timeouts",
     "fxenv_rollout_ex", "fxenv_policy_peek", "fxenv_set_reset_starts", "fxenv_get_episode_info",
     "fxenv_set_bracket_audit", "fxenv_get_bracket_audit", "fxenv_set_action_repeat", "fxenv_policy_create_ex",
+    "fxenv_set_time_limit",
 ]
 
 ROLLOUT_GREEDY = 1  # FXENV_ROLLOUT_GREEDY
 PEEK_OBS16, PEEK_H1 = 0, 1  # FXENV_PEEK_*
 MAX_REPEAT, REPEAT_HOLD = 256, 1  # FXENV_MAX_REPEAT, FXENV_REPEAT_HOLD
 POLICY_WIDTHS = (64, 128, 256, 512)  # the hidden widths fxenv_policy_create_ex accepts
+FLAG_TRUNCATED, TIME_LIMIT_WINDOW = 64, 1  # FX_FLAG_TRUNCATED, FXENV_TIME_LIMIT_WINDOW
+DONE_TERMINATED, DONE_TRUNCATED = 1, 2  # FXENV_DONE_* codes of the terminated / done outputs while truncation is on
 
 
 class FxEnvError(RuntimeError):
@@ -81,12 +84,12 @@ INFO_DTYPES = {
 
 def build(force: bool = False, verbose: bool = False) -> str:
     """Compile gym_fx_b200/csrc/*.cu into gym_fx_b200/libfxenv.so with nvcc for sm_90a (works without a GPU)."""
-    srcs = [os.path.join(CSRC, f) for f in ("fx_capi.cu", "fx_kernels.cu", "fx_policy.cu", "fx_core.cuh", "fx_kernels.cuh",
-                                            "fx_policy.cuh")]
+    srcs = [os.path.join(CSRC, f) for f in ("fx_capi.cu", "fx_kernels.cu", "fx_kernels_trunc.cu", "fx_policy.cu", "fx_core.cuh",
+                                            "fx_kernels.cuh", "fx_policy.cuh", "Makefile")]
     srcs.append(os.path.join(_HERE, "..", "include", "fxenv.h"))
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in srcs)
     if force or stale:
-        cmd = ["make", "-C", CSRC] + (["-B"] if force else [])
+        cmd = ["make", "-j4", "-C", CSRC] + (["-B"] if force else [])  # the sources compile in parallel
         out = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if verbose or out.returncode != 0:
             print(out.stdout)
@@ -144,6 +147,7 @@ def load():
     L.fxenv_set_bracket_audit.argtypes = [vp, C.c_int32]
     L.fxenv_get_bracket_audit.argtypes = [vp, C.POINTER(FxAuditPtrs)]
     L.fxenv_set_action_repeat.argtypes = [vp, C.c_int32, C.c_uint32]
+    L.fxenv_set_time_limit.argtypes = [vp, C.c_int32, C.c_uint32]
     if L.fxenv_abi_version() != 2:
         raise FxEnvError("libfxenv.so ABI version mismatch")
     _lib = L

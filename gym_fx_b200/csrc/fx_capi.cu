@@ -65,9 +65,10 @@ struct FxEnv {
     uint64_t used = 0;
   } graphs[2];
   uint64_t graph_clock = 0;
-  // bumped whenever a setting in the kernel parameters changes (the bracket audit, the action repeat): a cached rollout
+  // bumped whenever a setting in the kernel parameters changes (the bracket audit, the action repeat, the time limit): a cached rollout
   // graph captured the old P by value (FxPolicy::cached)
   uint64_t params_epoch = 0;
+  bool trunc_configured = false;   // fx_configure_trunc_kernels has run (fxenv_set_time_limit)
 };
 
 namespace {
@@ -223,6 +224,7 @@ int fxenv_create(const FxConfig* cfg, FxEnv** out) {
   o_sz = plan.add(N * capP * 8);
   const size_t o_ep_lo = plan.add(N * 8), o_ep_span = plan.add(N * 8), o_ep_seed = plan.add(8);
   const size_t o_ep_begun = plan.add(N * 4), o_ep_done = plan.add(N * 4), o_ep_last = plan.add(N * FXENV_EPISODE_STATS * 8);
+  const size_t o_ep_steps = plan.add(N * 4);
   env->slab_bytes = plan.bytes;
   ce = cudaMalloc(&env->slab, plan.bytes);
   if (ce != cudaSuccess) { fxenv_destroy(env); return cuda_fail(nullptr, ce, "cudaMalloc(state slab)"); }
@@ -254,6 +256,7 @@ int fxenv_create(const FxConfig* cfg, FxEnv** out) {
   st.ep_begun = reinterpret_cast<int32_t*>(b + o_ep_begun);
   st.ep_done = reinterpret_cast<int32_t*>(b + o_ep_done);
   st.ep_last = reinterpret_cast<double*>(b + o_ep_last);
+  env->P.ep_steps = reinterpret_cast<int32_t*>(b + o_ep_steps);
   *out = env;
   return FXENV_OK;
 }
@@ -643,6 +646,28 @@ int fxenv_set_action_repeat(FxEnv* env, int32_t repeat, uint32_t flags) {
   env->params_epoch++;   // ... and so did each policy's rollout graph
   env->P.repeat = repeat;
   env->P.repeat_flags = flags;
+  return FXENV_OK;
+}
+
+int fxenv_set_time_limit(FxEnv* env, int32_t max_steps, uint32_t flags) {
+  if (!env) return FXENV_E_INVALID;
+  if (max_steps < 0) return fail(env, FXENV_E_INVALID, "time limit must be >= 0 decisions, got " + std::to_string(max_steps));
+  if (flags & ~FXENV_TIME_LIMIT_WINDOW) return fail(env, FXENV_E_INVALID, "unknown time limit flags " + std::to_string(flags));
+  DeviceGuard g(env->device);
+  FX_CUDA(env, cudaDeviceSynchronize());  // no cached graph is destroyed, and no count zeroed, while a launch may run
+  drop_graph(env);       // the cached step-many graphs captured the old P
+  env->params_epoch++;   // ... and so did each policy's rollout graph
+  if ((max_steps > 0 || flags != 0u) && !env->trunc_configured) {
+    // the truncation kernels' first use on this handle: their attributes, and the persistent grid's minimum over them
+    // (every launch reads the grid and advances the ticket words by its own warp count)
+    FX_CUDA(env, fx_configure_trunc_kernels(env->P));
+    env->trunc_configured = true;
+  }
+  env->P.max_steps = max_steps;
+  env->P.trunc_flags = flags;
+  // every running episode starts counting from here
+  FX_CUDA(env, cudaMemset(env->P.ep_steps, 0, (size_t)env->P.cfg.num_envs * sizeof(int32_t)));
+  FX_CUDA(env, cudaDeviceSynchronize());
   return FXENV_OK;
 }
 

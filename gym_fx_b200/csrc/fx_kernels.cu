@@ -44,7 +44,18 @@ constexpr int kLongUnroll = FX_LONG_UNROLL;  // (a macro is not expanded inside 
 #ifndef FX_EMIT_EARLY
 #define FX_EMIT_EARLY 0  // 1: emit the observation windows right after the order sweep
 #endif
+// Time limit and truncation (include/fxenv.h, fxenv_set_time_limit): this file compiled with FX_KERNELS_TRUNC=1
+// (fx_kernels_trunc.cu) is the set of step / rollout instantiations that count decisions and report truncations.  The
+// host launches them only while fx_trunc_on(P); with truncation off the kernels of this translation unit run, and there
+// kTrunc is false, so they are exactly those of a build without the time limit.
+#ifndef FX_KERNELS_TRUNC
+#define FX_KERNELS_TRUNC 0
+#endif
+constexpr bool kTrunc = FX_KERNELS_TRUNC != 0;
 
+#if FX_KERNELS_TRUNC
+namespace fx_trunc {  // distinct kernel names in profiles
+#endif
 namespace {
 
 // per-warp shared memory: the TMA-staged candle window + z-score statistics (+ the Sharpe ring) + one mbarrier
@@ -78,6 +89,11 @@ enum {
 __device__ __forceinline__ int32_t* fx_carry_tab_hi(double* carry) {
   return reinterpret_cast<int32_t*>(carry + FX_CARRY_SHARPE_LAST) + 1;
 }
+
+// kTrunc: the carried decision count of the episode (the carry record's extra field) lives in the second half of the 16
+// bytes fx_warp_smem_bytes reserves for the 8-byte mbarrier, so that the slice -- and the kernels without truncation --
+// keep their size
+__device__ __forceinline__ int32_t* fx_carry_dec(const WarpSmem& ws) { return reinterpret_cast<int32_t*>(ws.bar + 1); }
 
 __host__ __device__ inline int fx_window_doubles(int W, int C) { return (W * C + 2 + 1) & ~1; }  // +1 alignment, even
 
@@ -214,7 +230,7 @@ __device__ __noinline__ void fx_reset_env(const FxKernelParams& P, const int env
     r[FXENV_EP_BARS] = (double)st.bar_index[env];
     r[FXENV_EP_EQUITY] = st.equity[env];
     r[FXENV_EP_COMMISSION] = st.commission_paid[env];
-    r[FXENV_EP_END_FLAGS] = (double)(flags & (FX_FLAG_TERMINATED | FX_FLAG_EXHAUSTED | FX_FLAG_BROKE));
+    r[FXENV_EP_END_FLAGS] = (double)(flags & (FX_FLAG_TERMINATED | FX_FLAG_EXHAUSTED | FX_FLAG_BROKE | FX_FLAG_TRUNCATED));
     r[FXENV_EP_DD_MAX_PCT] = rs[FX_RS_DD_MAX_PCT];
     r[FXENV_EP_DD_MAX_MONEY] = rs[FX_RS_DD_MAX_MONEY];
     r[FXENV_EP_PNL_NET] = rs[FX_RS_PNL_NET];
@@ -243,6 +259,7 @@ __device__ __noinline__ void fx_reset_env(const FxKernelParams& P, const int env
   st.n_orders[env] = 0;
   st.n_acc[env] = 0;
   st.sub_need[env] = 0.0;
+  P.ep_steps[env] = 0;
   for (int j = 0; j < FX_RS_N; j++) st.rstats[(int64_t)env * FX_RS_N + j] = (j == FX_RS_DD_MAXVALUE) ? c.initial_cash : 0.0;
   for (int j = 0; j < 5; j++) st.nbar[(int64_t)env * 6 + j] = tb.candles[start * (int64_t)c.n_cols + (j < 4 ? j : c.price_col)];
   if (fx_uses_running_stats(c)) {
@@ -772,6 +789,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   FxEnvRegs e;
   double2 nb_oh, nb_lc;
   double nb_price, rsv = 0.0;
+  int32_t dec = 0;  // kTrunc: decisions of the episode before this step
   if (CARRY && carry_in) {  // the record this warp left behind one step ago (shared memory: broadcast reads)
     const double* __restrict__ cr = ws.carry;
     const int2 ft = *reinterpret_cast<const int2*>(cr + FX_CARRY_FLAGS_T);
@@ -784,6 +802,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
     e.commission_paid = cr[FX_CARRY_COMM];
     nb_oh.x = cr[FX_CARRY_NBAR]; nb_oh.y = cr[FX_CARRY_NBAR + 1]; nb_lc.x = cr[FX_CARRY_NBAR + 2]; nb_lc.y = cr[FX_CARRY_NBAR + 3];
     nb_price = cr[FX_CARRY_NBAR + 4];
+    if (kTrunc) dec = *fx_carry_dec(ws);
 #ifndef FX_NO_RUN_STATS
     if (lane < FX_RS_N) rsv = cr[FX_CARRY_RSTATS + lane];
 #endif
@@ -801,6 +820,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
     const double2* __restrict__ nb2 = reinterpret_cast<const double2*>(st.nbar + (int64_t)env * 6);
     nb_oh = nb2[0]; nb_lc = nb2[1];
     nb_price = st.nbar[(int64_t)env * 6 + 4];
+    if (kTrunc) dec = P.ep_steps[env];
 #ifndef FX_NO_RUN_STATS
     if (lane < FX_RS_N) rsv = st.rstats[(int64_t)env * FX_RS_N + lane];  // DrawDown / TradeAnalyzer / SQN state
 #endif
@@ -836,8 +856,11 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   FX_STAMP_DEP(2, (unsigned long long)flags + (unsigned long long)t + (unsigned long long)start + (unsigned long long)total_bars);
 
   // ---- terminated envs: the reference answers (obs, 0.0, True) without touching plugins (app/env.py:137-138);
-  //      with auto_reset (build-side extension) the env restarts its episode window instead
-  if (flags & FX_FLAG_TERMINATED) {
+  //      with auto_reset (build-side extension) the env restarts its episode window instead.  A truncated env is
+  //      treated alike, answering FXENV_DONE_TRUNCATED -- also in the kernels without truncation: the flag is env state
+  //      and outlives the setting (a limit turned off, or a snapshot restored, before the cut env's reset step), and
+  //      its episode is over all the same (their 0 / 1 output then answers 1)
+  if (flags & (FX_FLAG_TERMINATED | FX_FLAG_TRUNCATED)) {
     if (RESIDENT && carry_in)  // this step returns false: the next one reloads the table from global memory
       fx_table_copy(st.o_meta + obase, st.o_p0 + obase, st.o_p1 + obase, st.o_sz + obase, gmeta, gp0, gp1, gsz,
                     *fx_carry_tab_hi(ws.carry), lane);
@@ -858,7 +881,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
     if (lane == 0) {
       reward[FX_OUT_IDX()] = 0.0f;
       if (reward64) reward64[FX_OUT_IDX()] = 0.0;
-      terminated[FX_OUT_IDX()] = c.auto_reset ? 0 : 1;
+      terminated[FX_OUT_IDX()] = c.auto_reset ? 0 : ((kTrunc && !(flags & FX_FLAG_TERMINATED)) ? FXENV_DONE_TRUNCATED : 1);
       fx_write_scalars<LEAN>(P, e, total_bars, tb.candles[(start + e.bar_index - 1) * (int64_t)C + c.price_col], FX_OBS_ROW(), FX_OBS_ROW16());
     }
     {
@@ -1116,7 +1139,10 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       fx_publish(e, b.c, t);
       if (e.equity <= c.min_equity) e.flags |= FX_FLAG_TERMINATED | FX_FLAG_BROKE;  // app/bt_bridge.py:140-143
     } else {
-      e.flags |= FX_FLAG_TERMINATED | FX_FLAG_EXHAUSTED;
+      // the episode window ran out: a truncation with FXENV_TIME_LIMIT_WINDOW (equity > min_equity here: an env at or
+      // below it terminated as broke on an earlier step)
+      e.flags |= (kTrunc && (P.trunc_flags & FXENV_TIME_LIMIT_WINDOW)) ? (FX_FLAG_EXHAUSTED | FX_FLAG_TRUNCATED)
+                                                                         : (FX_FLAG_TERMINATED | FX_FLAG_EXHAUSTED);
       e.prev_equity = st.prev_equity[env];
       e.bar_index = t + 1;
       e.position = e.psize > 0.0 ? 1 : (e.psize < 0.0 ? -1 : 0);
@@ -1163,10 +1189,15 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       }
     }
     const bool term = ((e.flags & FX_FLAG_TERMINATED) != 0u) || (e.equity <= c.min_equity);  // app/env.py:157
+    bool trunc = kTrunc && (e.flags & FX_FLAG_TRUNCATED) != 0u;  // the window ran out (FXENV_TIME_LIMIT_WINDOW)
     if (REPEAT) {  // the step's reward: the substeps' sum in substep order, from r0; a terminating substep ends the step
       if (sub->j > 0) r = sub->racc + r;
       sub->racc = r;
-      emit = emit || term;
+      emit = emit || term || trunc;
+    }
+    if (kTrunc && (!REPEAT || emit)) {  // one decision more; the limit cuts an episode that did not terminate
+      dec += 1;
+      if (!term && !trunc && P.max_steps > 0 && dec >= P.max_steps) { e.flags |= FX_FLAG_TRUNCATED; trunc = true; }
     }
     FX_STAMP(7);  // reward
 
@@ -1182,10 +1213,11 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       if (n_final != n) st.n_orders[env] = n_final;
       if (n_acc_new != n_acc) st.n_acc[env] = n_acc_new;
       if (sub_need_new != sub_need) st.sub_need[env] = sub_need_new;
+      if (kTrunc) P.ep_steps[env] = dec;
       if (!REPEAT || emit) {
         reward[FX_OUT_IDX()] = (float)r;
         if (reward64) reward64[FX_OUT_IDX()] = r;
-        terminated[FX_OUT_IDX()] = term ? 1 : 0;
+        terminated[FX_OUT_IDX()] = term ? 1 : ((kTrunc && trunc) ? FXENV_DONE_TRUNCATED : 0);
         fx_write_scalars<LEAN>(P, e, total_bars, last_price, FX_OBS_ROW(), FX_OBS_ROW16());
       }
       if (CARRY) {  // what the env's next step starts from, should this warp run it (the arrays above stay authoritative)
@@ -1196,6 +1228,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
         *reinterpret_cast<int2*>(cr + FX_CARRY_BARS_N) = make_int2(total_bars, n_final);
         *reinterpret_cast<int2*>(cr + FX_CARRY_NACC_TRADES) = make_int2(n_acc_new, e.trades);
         *reinterpret_cast<long long*>(cr + FX_CARRY_START) = start;
+        if (kTrunc) *fx_carry_dec(ws) = dec;
         if (RESIDENT) {  // every index this ticket wrote is below the largest table size it saw: the write-back range,
                          // which leaves the global arrays exactly as the global-table kernel does (stale entries included)
           int32_t* hi = fx_carry_tab_hi(cr);
@@ -1423,6 +1456,7 @@ fx_rollout_kernel(const __grid_constant__ FxKernelParams P, const char* __restri
   }
 }
 
+#if !FX_KERNELS_TRUNC  // the kernels below and the host code have one copy, in fx_kernels.cu
 __global__ void fx_reset_kernel(const __grid_constant__ FxKernelParams P, const int64_t* __restrict__ start_bar,
                                 const uint8_t* __restrict__ mask, int first) {
   const int env = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1485,9 +1519,10 @@ __global__ void fx_stats_kernel(FxConfig c, const double* __restrict__ candles, 
   stats[idx * 2 + 0] = m;
   stats[idx * 2 + 1] = rc;
 }
+#endif  // !FX_KERNELS_TRUNC
 
-typedef void (*StepKernel)(const FxKernelParams, const void*, float*, float*, double*, uint8_t*, int, int, uint16_t*, int, const FxTileSync);
-typedef void (*RolloutKernel)(const FxKernelParams, const char*, float*, int, float*, uint8_t*, const FxChunkPlan, unsigned, unsigned);
+typedef FxStepKernelFn StepKernel;
+typedef FxRolloutKernelFn RolloutKernel;
 
 // mode: 0 = general features, 1 = 5-feature fast path, 2 = LEAN (implies the 5-feature fast path)
 template <int STRAT, int REWARD>
@@ -1533,7 +1568,13 @@ int kernel_strat(const FxKernelParams& P, int audit, int repeat) {
   return s;
 }
 
-StepKernel pick_kernel(const FxKernelParams& P, int lean = -1, int audit = -1, int repeat = -1) {
+// trunc: as audit / repeat, for the truncation instantiations (fx_kernels_trunc.cu)
+StepKernel pick_kernel(const FxKernelParams& P, int lean = -1, int audit = -1, int repeat = -1, int trunc = -1) {
+#if !FX_KERNELS_TRUNC
+  if (trunc < 0 ? fx_trunc_on(P) : trunc != 0) return fx_pick_step_trunc(P, lean, audit, repeat);
+#else
+  (void)trunc;
+#endif
   const int mode = kernel_mode(P, lean < 0 ? P.lean : lean);
   const int r = P.cfg.reward;
   switch (kernel_strat(P, audit, repeat)) {
@@ -1548,7 +1589,12 @@ StepKernel pick_kernel(const FxKernelParams& P, int lean = -1, int audit = -1, i
   }
 }
 
-RolloutKernel pick_rollout(const FxKernelParams& P, int lean = -1, int audit = -1, int repeat = -1) {
+RolloutKernel pick_rollout(const FxKernelParams& P, int lean = -1, int audit = -1, int repeat = -1, int trunc = -1) {
+#if !FX_KERNELS_TRUNC
+  if (trunc < 0 ? fx_trunc_on(P) : trunc != 0) return fx_pick_rollout_trunc(P, lean, audit, repeat);
+#else
+  (void)trunc;
+#endif
   const int mode = kernel_mode(P, lean < 0 ? P.lean : lean);
   const bool res = P.order_smem != 0;
   const int r = P.cfg.reward;
@@ -1564,6 +1610,7 @@ RolloutKernel pick_rollout(const FxKernelParams& P, int lean = -1, int audit = -
   }
 }
 
+#if !FX_KERNELS_TRUNC
 size_t step_smem_bytes(const FxKernelParams& P) {
   const int ring_len = (P.cfg.reward == FX_REWARD_SHARPE) ? P.cfg.sharpe_window : 0;
   return fx_warp_smem_bytes(fx_window_doubles(P.cfg.window_size, P.cfg.n_cols), ring_len) * FX_WARPS;
@@ -1590,8 +1637,20 @@ int carveout_pct(size_t ctas, size_t smem) {
   if (const char* cv = getenv("FXENV_CARVEOUT")) { const int v = atoi(cv); if (v >= pct && v <= 100) pct = v; }  // measurements
   return pct;
 }
+#endif  // !FX_KERNELS_TRUNC
 
 }  // namespace
+
+#if FX_KERNELS_TRUNC
+}  // namespace fx_trunc
+
+FxStepKernelFn fx_pick_step_trunc(const FxKernelParams& P, int lean, int audit, int repeat) {
+  return fx_trunc::pick_kernel(P, lean, audit, repeat);
+}
+FxRolloutKernelFn fx_pick_rollout_trunc(const FxKernelParams& P, int lean, int audit, int repeat) {
+  return fx_trunc::pick_rollout(P, lean, audit, repeat);
+}
+#else
 
 // The resident-table rollout kernel when its CTAs fit an SM as many warps as the global-table one runs (16): each
 // CTA at most 227 KB, and (16 / FX_ROLLOUT_WARPS(true)) CTAs plus their 1 KB reservations at most the SM's 228 KB.
@@ -1603,30 +1662,22 @@ int fx_order_smem_choice(const FxKernelParams& P, int force) {
   return (cta <= 227 * 1024 && ctas * (cta + 1024) <= 228 * 1024) ? 1 : 0;
 }
 
-// dynamic shared memory above the 48 KB default needs an explicit opt-in per kernel
-cudaError_t fx_configure_kernels(FxKernelParams& P) {
-  const size_t smem = step_smem_bytes(P);
-  if (smem > 227 * 1024) return cudaErrorInvalidValue;
-  const char* os = getenv("FXENV_ORDER_SMEM");
-  P.order_smem = fx_order_smem_choice(P, os ? atoi(os) : -1);
-  const size_t rsmem = rollout_smem_bytes(P, P.order_smem != 0);
-  if (rsmem > 227 * 1024) return cudaErrorInvalidValue;
+// Attributes of one set of step / rollout instantiations (trunc: the truncation twins) and the persistent grid: dynamic
+// shared memory above the 48 KB default needs an explicit opt-in per kernel.  P.order_smem is decided.
+static cudaError_t fx_configure_variants(FxKernelParams& P, int trunc) {
+  const size_t smem = step_smem_bytes(P), rsmem = rollout_smem_bytes(P, P.order_smem != 0);
   // ask for enough shared-memory carve-out that FX_MIN_BLOCKS CTAs (+1 KB system use each) fit on an SM
   const int pct = carveout_pct(FX_MIN_BLOCKS, smem);
   const int rcta = rollout_cta_warps(P);
   const int rpct = carveout_pct((size_t)FX_ROLLOUT_MIN_BLOCKS * FX_WARPS / rcta, rsmem);
-  int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  P.num_sms = sms > 0 ? sms : 1;
-  P.resident_blocks = 0;
+  const int sms = P.num_sms;
   // both the general and the LEAN instantiation: which one runs is only known once the candle tables are loaded; for
   // the ATR strategy also both states of the bracket audit; and both states of the action repeat
   const int n_lean = P.fast_features == 5 ? 2 : 1, n_audit = P.cfg.strategy == FX_STRATEGY_ATR_SLTP ? 2 : 1;
   for (int v = 0; v < n_lean * n_audit * 2; v++) {
     const int lean = v % n_lean, audit = (v / n_lean) % n_audit, repeat = v / (n_lean * n_audit);
-    const StepKernel sk = pick_kernel(P, lean, audit, repeat);
-    const RolloutKernel rk = pick_rollout(P, lean, audit, repeat);
+    const StepKernel sk = pick_kernel(P, lean, audit, repeat, trunc);
+    const RolloutKernel rk = pick_rollout(P, lean, audit, repeat, trunc);
     cudaError_t e = cudaFuncSetAttribute(sk, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
     if (e != cudaSuccess) return e;
     e = cudaFuncSetAttribute(rk, cudaFuncAttributePreferredSharedMemoryCarveout, rpct);
@@ -1640,18 +1691,35 @@ cudaError_t fx_configure_kernels(FxKernelParams& P) {
       if (e != cudaSuccess) return e;
     }
     // how many CTAs of the persistent rollout kernel the device holds at once (= its grid size).  The minimum over every
-    // variant configured here, the bracket audit's and the action repeat's included: one grid size serves whichever
-    // variant a launch picks, so a change that raises those kernels' registers or shared memory shrinks the grid with
-    // them off as well
+    // variant configured so far, the bracket audit's and the action repeat's included (the truncation's once a limit is
+    // set): one grid size serves whichever variant a launch picks, so a change that raises those kernels' registers or
+    // shared memory shrinks the grid with them off as well
     int per_sm = 0;
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rk, rcta * 32, rsmem);
     if (e != cudaSuccess) return e;
     if (P.resident_blocks == 0 || sms * per_sm < P.resident_blocks) P.resident_blocks = sms * per_sm;
   }
-  if (P.resident_blocks < 1) return cudaErrorInvalidConfiguration;
+  return P.resident_blocks < 1 ? cudaErrorInvalidConfiguration : cudaSuccess;
+}
+
+cudaError_t fx_configure_kernels(FxKernelParams& P) {
+  const size_t smem = step_smem_bytes(P);
+  if (smem > 227 * 1024) return cudaErrorInvalidValue;
+  const char* os = getenv("FXENV_ORDER_SMEM");
+  P.order_smem = fx_order_smem_choice(P, os ? atoi(os) : -1);
+  if (rollout_smem_bytes(P, P.order_smem != 0) > 227 * 1024) return cudaErrorInvalidValue;
+  int dev = 0, sms = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  P.num_sms = sms > 0 ? sms : 1;
+  P.resident_blocks = 0;
+  const cudaError_t e = fx_configure_variants(P, 0);
+  if (e != cudaSuccess) return e;
   if (smem <= 48 * 1024) return cudaSuccess;
   return cudaFuncSetAttribute(fx_observe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)observe_smem_bytes(P));
 }
+
+cudaError_t fx_configure_trunc_kernels(FxKernelParams& P) { return fx_configure_variants(P, 1); }
 
 // The LEAN contract of the specialised kernels (see fx_uses_running_stats): everything here is a property of the
 // resolved configuration except `tame_data`, which is known once every pair's candle table has been loaded.
@@ -1764,3 +1832,4 @@ cudaError_t fx_launch_stats(const FxConfig& cfg, const double* candles, double* 
   fx_stats_kernel<<<(unsigned)((total + threads - 1) / threads), threads, 0, stream>>>(cfg, candles, stats, T);
   return cudaGetLastError();
 }
+#endif  // FX_KERNELS_TRUNC

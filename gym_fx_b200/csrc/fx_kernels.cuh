@@ -86,7 +86,16 @@ struct FxKernelParams {
   // FXENV_REPEAT_* flags.  A setting of the handle, not env state: outside the slab, like the audit.
   int32_t repeat;
   uint32_t repeat_flags;
+  // time limit (fxenv_set_time_limit): decisions per episode (0 = no limit) and the FXENV_TIME_LIMIT_* flags.  A setting
+  // of the handle like the repeat; while either is set the host launches the truncation instantiations (fx_trunc_on).
+  int32_t max_steps;
+  uint32_t trunc_flags;
+  // [N] decisions of the current episode (a column of the state slab, so snapshots carry it; zeroed by fx_reset_env).
+  // Addressed from here rather than from FxDeviceState so that no existing kernel parameter moves.
+  int32_t* ep_steps;
 };
+
+__host__ __device__ inline bool fx_trunc_on(const FxKernelParams& P) { return P.max_steps > 0 || P.trunc_flags != 0u; }
 
 // warps (= envs) per CTA of the step kernel.  One warp per CTA lets the second wave back-fill SM slots as soon as a
 // single env finishes.
@@ -134,6 +143,9 @@ cudaError_t fx_launch_observe(const FxKernelParams& P, float* obs, cudaStream_t 
                               int stride16 = 0);
 cudaError_t fx_launch_stats(const FxConfig& cfg, const double* candles, double* stats, int64_t T, cudaStream_t stream);
 cudaError_t fx_configure_kernels(FxKernelParams& P);
+// the same for the truncation instantiations; deferred to the first fxenv_set_time_limit that turns truncation on, so
+// that a handle without a time limit never loads their module
+cudaError_t fx_configure_trunc_kernels(FxKernelParams& P);
 bool fx_config_is_lean(const FxKernelParams& P);
 cudaError_t fx_launch_rollout(const FxKernelParams& P, const void* actions, float* obs, int obs_slots, float* reward,
                               uint8_t* terminated, const FxChunkPlan& plan, unsigned seq_base, unsigned ticket_base,
@@ -141,4 +153,12 @@ cudaError_t fx_launch_rollout(const FxKernelParams& P, const void* actions, floa
 int fx_rollout_blocks(const FxKernelParams& P);
 int fx_rollout_warps(const FxKernelParams& P);  // warps of a fx_rollout_kernel launch (each draws one ticket past the last)
 int fx_order_smem_choice(const FxKernelParams& P, int force);
+// the truncation instantiations (fx_kernels_trunc.cu: fx_kernels.cu compiled with FX_KERNELS_TRUNC), picked by
+// fx_kernels.cu while fx_trunc_on(P); lean / audit / repeat as in its pick_kernel / pick_rollout
+typedef void (*FxStepKernelFn)(const FxKernelParams, const void*, float*, float*, double*, uint8_t*, int, int, uint16_t*, int,
+                               const FxTileSync);
+typedef void (*FxRolloutKernelFn)(const FxKernelParams, const char*, float*, int, float*, uint8_t*, const FxChunkPlan, unsigned,
+                                  unsigned);
+FxStepKernelFn fx_pick_step_trunc(const FxKernelParams& P, int lean, int audit, int repeat);
+FxRolloutKernelFn fx_pick_rollout_trunc(const FxKernelParams& P, int lean, int audit, int repeat);
 FxChunkPlan fx_rollout_plan(const FxKernelParams& P, int n_steps);  // the host's ticket accounting needs n_rounds

@@ -12,6 +12,10 @@ Differences, all deliberate (SURVEY.md App. B):
   * there is no backtrader: `summary()` passes an empty analyzers dict to the metrics plugin, which is what the
     reference effectively does on the live path (App. B #12).
 
+With the config key `max_episode_steps` (Gymnasium's name; not a reference key) an episode is cut after that many steps:
+step() then returns terminated=False, truncated=True, and keeps answering so until reset(), as after a termination.
+Without the key, truncated is always False as in the reference.
+
 With direct_atr_sltp and GYMFX_BRACKET_AUDIT set (read at import of the strategy module, as in the reference), every
 step() appends the decisions the step kernel logged to that file, in the reference's line format.
 """
@@ -69,6 +73,11 @@ class GymFxEnv(spaces.EnvBase):
                                    columns=self._columns, num_envs=1,
                                    order_capacity=int(cfg.get("order_capacity", 256)))
 
+        mes = cfg.get("max_episode_steps")
+        if mes is not None and (isinstance(mes, bool) or int(mes) != mes or int(mes) < 1):
+            raise ValueError(f"max_episode_steps must be a positive integer, got {mes!r}")
+        self.max_episode_steps = None if mes is None else int(mes)
+
         self.action_space_mode = str(cfg.get("action_space_mode", "discrete")).lower()
         if self.action_space_mode == "continuous":
             self.action_space = spaces.Box(low=-1.0, high=1.0, shape=(1,), dtype=np.float32)
@@ -102,6 +111,8 @@ class GymFxEnv(spaces.EnvBase):
             self._vec = VecFxEnv(self._fxcfg, [self._table], [self._minutes])
             if _atr._AUDIT_PATH and self._fxcfg.strategy == STRATEGY_ATR_SLTP:
                 self._vec.set_bracket_audit(4)  # at most one record per step, drained after every step
+            if self.max_episode_steps is not None:
+                self._vec.set_time_limit(self.max_episode_steps)
         obs, _ = self._vec.reset(torch.zeros(1, dtype=torch.int64))
         self._started = True
         self._terminated = False
@@ -115,18 +126,18 @@ class GymFxEnv(spaces.EnvBase):
             raise RuntimeError("Call reset() before step().")
         was_terminated = self._terminated
         a = torch.tensor([self._host_action(action)], dtype=self._vec.action_dtype, device=self._vec.device)
-        obs, _, term, _, _ = self._vec.step(a)
+        obs, _, term, trunc, _ = self._vec.step(a)
         if self._vec._audit is not None:
             self._emit_audit()
         reward = float(self._vec.reward64[0])          # fp64, like the reference's Python float
-        terminated = bool(term[0])
-        self._terminated = terminated
+        terminated, truncated = bool(term[0]), bool(trunc[0])
+        self._terminated = terminated or truncated  # the episode is over either way
         info = self._make_info()
         pnl = info.pop("_pnl")
         self._last_equity = info["equity"]
         if not was_terminated:  # a step on an already terminated env returns the bare _make_info() (app/env.py:137-138)
             info.update(reward=reward, pnl=pnl, trade_cost=0.0)  # trade_cost is always 0.0 (App. B #7)
-        return self._split(obs[0].cpu().numpy()), reward, terminated, False, info
+        return self._split(obs[0].cpu().numpy()), reward, terminated, truncated, info
 
     def render(self):
         return None
@@ -173,7 +184,7 @@ class GymFxEnv(spaces.EnvBase):
     def summary(self) -> Dict[str, Any]:
         """app/env.py:256-271.  The reference sees its analyzers only once cerebro.run() has returned -- i.e. after the
         episode terminated (data exhausted / broke) or after close() -- and an empty dict before (SURVEY App. B #12);
-        the same rule is kept here, with the analyzer results coming from the step kernel's per-env statistics."""
+        the same rule is kept here (an episode cut by max_episode_steps counts as ended), with the analyzer results coming from the step kernel's per-env statistics."""
         final = float(self._vec.info()["equity"][0]) if self._vec is not None else self._last_equity
         analyzers: Dict[str, Any] = {}
         if self._vec is not None and self._terminated:

@@ -10,6 +10,10 @@ learned policy -- written in plain torch (autograd for the backward pass):
 Auto-reset semantics (include/fxenv.h, FxConfig.auto_reset): the step AFTER a termination is a reset step -- its action
 is ignored, its reward is 0 and its observation jumps to the new episode.  Those transitions carry no learning signal
 and are masked out of the advantage statistics and of the loss; `done[t]` cuts the GAE recursion at t.
+With a time limit (VecFxEnv.set_time_limit) `done` holds codes: 1 = terminated, 2 = truncated.  A truncation also cuts
+the recursion and masks the reset step after it, but its TD target keeps gamma * V(final observation) -- value[t + 1],
+the value of the cut episode's last observation -- because the episode did not end in the MDP (Pardo et al., "Time
+Limits in Reinforcement Learning", 2018).
 """
 from __future__ import annotations
 
@@ -57,20 +61,23 @@ def gaussian_entropy(log_std):
 
 
 def gae(reward, value, done, prev_done, gamma: float = 0.99, lam: float = 0.95):
-    """-> (advantage [H, N], return [H, N], valid [H, N]).  value is [H + 1, N]; prev_done [N] = done flag of the step
-    before this rollout (1 where step 0 is a reset step)."""
+    """-> (advantage [H, N], return [H, N], valid [H, N]).  value is [H + 1, N]; done [H, N] the 0 / 1 flags or the codes
+    0 / 1 = terminated / 2 = truncated; prev_done [N] = done flag or code of the step before this rollout (non-zero where
+    step 0 is a reset step).  Any non-zero done[t] cuts the recursion at t and masks step t + 1; only a termination
+    drops gamma * value[t + 1] from delta_t, a truncation bootstraps from it."""
     H = reward.shape[0]
     adv = torch.zeros_like(reward)
     last = torch.zeros_like(reward[0])
-    donef = done.to(reward.dtype)
+    cut = (done != 0).to(reward.dtype)
+    boot = (done != 1).to(reward.dtype)   # 1 - terminated (FXENV_DONE_TERMINATED == 1)
     for t in reversed(range(H)):
-        nd = 1.0 - donef[t]
-        delta = reward[t] + gamma * value[t + 1] * nd - value[t]
+        nd = 1.0 - cut[t]
+        delta = reward[t] + gamma * value[t + 1] * boot[t] - value[t]
         last = delta + gamma * lam * nd * last
         adv[t] = last
     valid = torch.ones_like(reward)
-    valid[0] = 1.0 - prev_done.to(reward.dtype)
-    valid[1:] = 1.0 - donef[:-1]
+    valid[0] = 1.0 - (prev_done != 0).to(reward.dtype)
+    valid[1:] = 1.0 - cut[:-1]
     return adv, adv + value[:H], valid
 
 

@@ -57,7 +57,8 @@ class VecFxEnv:
         self.reward = torch.empty(N, dtype=torch.float32, device=dev)
         self.reward64 = torch.empty(N, dtype=torch.float64, device=dev)
         self.terminated = torch.empty(N, dtype=torch.uint8, device=dev)
-        self.truncated = torch.zeros(N, dtype=torch.bool, device=dev)  # always False (app/env.py:158)
+        self.truncated = torch.zeros(N, dtype=torch.bool, device=dev)  # always False (app/env.py:158) without a time limit
+        self._term_bool = None  # bool [N] split of the codes while truncation is on (set_time_limit)
         self._info_ptrs = _native.FxInfoPtrs()
         self.L.fxenv_get_info(self._h, C.byref(self._info_ptrs))
         self._info_views: Dict[str, torch.Tensor] = {}
@@ -65,6 +66,7 @@ class VecFxEnv:
         self._policies: list = []
         self._audit = None  # (ring [N, capacity, 8], written [N], read cursor [N]) while the bracket audit is on
         self.action_repeat = (1, False)  # (k, hold): set_action_repeat
+        self.time_limit = (0, False)  # (max_steps, truncate_window): set_time_limit
 
     # ------------------------------------------------------------------ lifecycle
     def close(self):
@@ -109,6 +111,7 @@ class VecFxEnv:
     def step(self, actions: torch.Tensor, out_obs: Optional[torch.Tensor] = None):
         """-> (obs, reward float32 [N], terminated bool [N], truncated bool [N], info).
         One step is one decision: with an action repeat k > 1 (set_action_repeat) it runs up to k bars.
+        truncated is all False unless a time limit is set (set_time_limit); terminated and truncated are never both True.
         The returned tensors are views of buffers that the next step() overwrites."""
         a = actions
         if a.dtype != self.action_dtype or a.device != self.device or not a.is_contiguous():
@@ -123,7 +126,12 @@ class VecFxEnv:
         rc = self.L.fxenv_step(self._h, a.data_ptr(), obs.data_ptr(), self.reward.data_ptr(),
                                self.terminated.data_ptr(), self.reward64.data_ptr(), self._stream())
         _native.check(self.L, self._h, rc, "fxenv_step")
-        return obs, self.reward, self.terminated.view(torch.bool), self.truncated, self.info()
+        if self._term_bool is None:
+            return obs, self.reward, self.terminated.view(torch.bool), self.truncated, self.info()
+        # truncation on: self.terminated holds the FXENV_DONE_* codes
+        torch.eq(self.terminated, _native.DONE_TERMINATED, out=self._term_bool)
+        torch.eq(self.terminated, _native.DONE_TRUNCATED, out=self.truncated)
+        return obs, self.reward, self._term_bool, self.truncated, self.info()
 
     # ---- argument checks of the raw-pointer calls: a wrong dtype / shape / device would be read as garbage or fault
     def _check(self, name: str, t: torch.Tensor, dtype: torch.dtype, shape, host: bool = False):
@@ -158,7 +166,8 @@ class VecFxEnv:
     def step_many(self, actions: torch.Tensor, obs_ring: torch.Tensor, rewards: torch.Tensor, terminated: torch.Tensor):
         """K consecutive steps with all actions supplied up front (replay / random / scripted drivers); identical results
         to K calls of step().  A step is a decision (up to k bars with set_action_repeat).  actions [K, N] (int32, or float32 in continuous mode); obs_ring float32 [slots, N, D]
-        (step k writes slot k % slots); rewards float32 [K, N]; terminated uint8 [K, N].  The library runs the batch as one
+        (step k writes slot k % slots); rewards float32 [K, N]; terminated uint8 [K, N]: 0 / 1, or with a time limit
+        (set_time_limit) the codes 0, 1 = terminated, 2 = truncated.  The library runs the batch as one
         persistent launch or as a cached CUDA graph of single steps (`step_many_engine`)."""
         K = self._check_batch(actions, obs_ring, rewards, terminated)
         rc = self.L.fxenv_step_many(self._h, K, actions.data_ptr(), obs_ring.data_ptr(), int(obs_ring.shape[0]),
@@ -343,8 +352,8 @@ class VecFxEnv:
         """The record of each env's last finished episode (latched when a reset -- auto or explicit -- ended it), as device
         tensors: what RecordEpisodeStatistics / GymFxEnv.summary() would report for it.  `episodes_done` counts the
         records (0: nothing recorded yet, the fields are then 0); `start` is the first bar of the CURRENT episode,
-        `episode_start` that of the recorded one.  end_flags: FX_FLAG_TERMINATED | EXHAUSTED | BROKE bits, 0 = cut short
-        by a reset.  total_return, avg_trade_pnl (NaN without closed trades) and sqn are derived as in summary()."""
+        `episode_start` that of the recorded one.  end_flags: FX_FLAG_TERMINATED (2) | EXHAUSTED (4) | BROKE (8) |
+        TRUNCATED (64) bits, 0 = cut short by a reset.  total_return, avg_trade_pnl (NaN without closed trades) and sqn are derived as in summary()."""
         start, done, last = self._episode_views()
         E = _native.EP
         col = {k: last[:, j] for k, j in E.items()}
@@ -432,6 +441,36 @@ class VecFxEnv:
         _native.check(self.L, self._h, rc, "fxenv_set_action_repeat")
         self.action_repeat = (k, bool(hold))
 
+    # ------------------------------------------------------------------ time limit / truncation
+    def set_time_limit(self, max_steps: int, truncate_window: bool = False):
+        """End every episode after `max_steps` decisions as a truncation (Gymnasium's max_episode_steps; 0 = no limit,
+        the default), and with truncate_window=True report the end of the episode window (episode_bars or the end of the
+        table) as a truncation instead of a termination.  A decision is one step(), step_many() decision or rollout()
+        decision; the first step of an episode is decision 1, an auto-reset step does not count.  A step that terminates
+        (broke) reports a termination only.  While either is set, step() returns real truncated flags and the uint8
+        outputs of step_many / step_host / rollout (done) carry codes 0, 1 = terminated, 2 = truncated.  Every running
+        episode starts counting afresh.  A setting of the handle (include/fxenv.h fxenv_set_time_limit): snapshots and
+        reset() keep it; each env's decision count is env state.  Synchronous."""
+        if isinstance(max_steps, bool) or int(max_steps) != max_steps:
+            raise ValueError(f"time limit must be an integer, got {max_steps!r}")
+        max_steps = int(max_steps)
+        if not 0 <= max_steps < 2**31:
+            raise ValueError(f"time limit must be in [0, 2**31), got {max_steps}")
+        if not isinstance(truncate_window, bool):
+            raise ValueError(f"truncate_window must be a bool, got {truncate_window!r}")
+        with torch.cuda.device(self.device):
+            rc = self.L.fxenv_set_time_limit(self._h, max_steps, _native.TIME_LIMIT_WINDOW if truncate_window else 0)
+        if rc == -1:
+            raise ValueError(self.L.fxenv_last_error(self._h).decode())
+        _native.check(self.L, self._h, rc, "fxenv_set_time_limit")
+        self.time_limit = (max_steps, truncate_window)
+        if max_steps > 0 or truncate_window:
+            if self._term_bool is None:
+                self._term_bool = torch.zeros(self.num_envs, dtype=torch.bool, device=self.device)
+        else:   # off: back to the zero-overhead views of the 0 / 1 buffer
+            self._term_bool = None
+            self.truncated.zero_()
+
     # ------------------------------------------------------------------ closed loop (policy on the device)
     def make_policy(self, weights=None, hidden: Optional[int] = None) -> "FusedPolicy":
         """An actor-critic MLP(obs_dim, hidden, hidden) evaluated by the fused tensor-core kernel (fxenv.h: FxPolicy).
@@ -445,7 +484,9 @@ class VecFxEnv:
         loop of the reference's driver (app/main.py:57-65) with a learned policy.  A step is one policy decision: with an
         action repeat k > 1 (set_action_repeat) the env runs up to k bars between two evaluations.  Returns / fills `buffers`:
         obs [H+1, N, D] (obs[t] is what the policy saw at step t), actions [H, N] (int32, or float32 in continuous mode),
-        logp [H, N], value [H+1, N] (value[H] bootstraps), reward [H, N], done uint8 [H, N].
+        logp [H, N], value [H+1, N] (value[H] bootstraps), reward [H, N], done uint8 [H, N] (0 / 1, or with a time limit
+        the codes 0, 1 = terminated, 2 = truncated: after a truncation at t, obs[t+1] is the final observation of the
+        cut episode, value[t+1] its value, and step t+1 the reset step with auto_reset).
         Sampling noise for reproducible rollouts -- discrete mode: gumbel, float32 [H, N, 3] Gumbel(0,1); continuous
         mode: noise, float32 [H, N] standard normal; default: the kernel's counter-based generator seeded with `seed`.
         deterministic: greedy evaluation, the most likely action (argmax of the logits / the Gaussian mean)."""

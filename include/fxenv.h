@@ -21,6 +21,7 @@
  *   fxenv_rollout / fxenv_rollout_ex  the caller loop of app/main.py:57-65 with a learned policy (see below);
  *                                  continuous actions are the Box(-1, 1, (1,)) of app/env.py:71-80, 187-204
  *   fxenv_set_action_repeat        (no counterpart: k bars per step, one decision per step; its contract below)
+ *   fxenv_set_time_limit           (no counterpart: Gymnasium's max_episode_steps and truncation; its contract below)
  *
  * Conventions: every function returns 0 on success, <0 on error (see FXENV_E_*); fxenv_last_error() gives the
  * message.  No exceptions or aborts cross the ABI.  The library owns env state (device struct-of-arrays) behind
@@ -65,6 +66,7 @@ enum { FX_SIZE_FX_UNITS = 0, FX_SIZE_NOTIONAL = 1 };
 #define FX_FLAG_BROKE 8u          /* equity <= min_equity                 app/bt_bridge.py:203-204 */
 #define FX_FLAG_ORDER_OVERFLOW 16u/* order table full: an order was dropped (the reference is unbounded) */
 #define FX_FLAG_TRADE_PRICE_OWN 32u /* statistics bookkeeping: the open trade's average price differs from the position's */
+/* FX_FLAG_TRUNCATED (64u): see fxenv_set_time_limit */
 
 /*
  * The reference resolves one "dict of everything" at call time (app/config.py:1-45, plugin_params of every
@@ -261,7 +263,8 @@ enum {
   FXENV_EP_BARS,            /* bars it ran (bridge.bar_index) */
   FXENV_EP_EQUITY,          /* final equity */
   FXENV_EP_COMMISSION,      /* commission paid */
-  FXENV_EP_END_FLAGS,       /* flags & (FX_FLAG_TERMINATED | FX_FLAG_EXHAUSTED | FX_FLAG_BROKE); 0 = cut short by a reset */
+  FXENV_EP_END_FLAGS,       /* flags & (FX_FLAG_TERMINATED | FX_FLAG_EXHAUSTED | FX_FLAG_BROKE | FX_FLAG_TRUNCATED);
+                             * 0 = cut short by a reset */
   FXENV_EP_DD_MAX_PCT,      /* drawdown.max.drawdown (percent) */
   FXENV_EP_DD_MAX_MONEY,    /* drawdown.max.moneydown */
   FXENV_EP_PNL_NET,         /* trades.pnl.net.total */
@@ -349,6 +352,35 @@ int fxenv_get_bracket_audit(FxEnv* env, FxAuditPtrs* out);
 #define FXENV_MAX_REPEAT 256
 #define FXENV_REPEAT_HOLD 1u
 int fxenv_set_action_repeat(FxEnv* env, int32_t repeat, uint32_t flags);
+
+/* ---- time limit and truncation: an episode cut short is reported as truncated, not terminated (no reference
+ * counterpart: Gymnasium's max_episode_steps / TimeLimit; a learner bootstraps through a truncation) ----------------
+ * max_steps > 0 ends an episode at the end of its max_steps-th DECISION: one step of fxenv_step / fxenv_step_host, one
+ * decision of fxenv_step_many / fxenv_rollout (with an action repeat k it spans up to k bars).  The first step of an
+ * episode (it does not advance the bar) is decision 1; an auto-reset step belongs to neither episode and does not
+ * count.  max_steps = 0: no limit.  FXENV_TIME_LIMIT_WINDOW: the step that finds the episode window exhausted (at
+ * FxConfig.episode_bars or at the end of the table) sets FX_FLAG_EXHAUSTED | FX_FLAG_TRUNCATED instead of
+ * FX_FLAG_EXHAUSTED | FX_FLAG_TERMINATED.  Broke stays a termination.
+ *   Precedence: a decision that terminates the episode (broke, or exhaustion without the WINDOW flag) reports a
+ *     termination only, even if it also reaches the limit.  FX_FLAG_TRUNCATED and FX_FLAG_TERMINATED are never set
+ *     together.
+ *   After a truncation the env behaves exactly as after a termination: with auto_reset the next step is the reset
+ *     step (the new episode, reward 0, code 0); without it every later step returns the same observation, reward 0 and
+ *     FXENV_DONE_TRUNCATED.
+ *   Outputs: while truncation is on (max_steps > 0 or the WINDOW flag), the uint8 terminated / done output of
+ *     fxenv_step, fxenv_step_host, fxenv_step_many and FxRollout.done carries a code: 0, FXENV_DONE_TERMINATED or
+ *     FXENV_DONE_TRUNCATED (non-zero still means "episode over").  While it is off they are 0 / 1 as without it.
+ *   State: each env counts the decisions of its episode in the env state (snapshots carry the count; a reset zeroes
+ *     it).  The limit and the flags belong to the handle, like the action repeat: fxenv_state_bytes, snapshots,
+ *     fxenv_reset and fxenv_set_state neither include nor change them.
+ * Synchronous.  Zeroes every env's decision count (an episode already running gets max_steps more decisions), drops the
+ * cached step-many graphs and makes each policy re-capture its rollout graph.  max_steps < 0 or unknown flag bits:
+ * FXENV_E_INVALID. */
+#define FX_FLAG_TRUNCATED 64u          /* the episode was cut by the time limit / window (above); never with TERMINATED */
+#define FXENV_TIME_LIMIT_WINDOW 1u     /* data exhaustion of the episode window is a truncation, not a termination */
+#define FXENV_DONE_TERMINATED 1
+#define FXENV_DONE_TRUNCATED 2
+int fxenv_set_time_limit(FxEnv* env, int32_t max_steps, uint32_t flags);
 
 /* ---- closed loop: a policy on the device between the steps ------------------------------------------------------
  * Replaces the caller loop of app/main.py:57-65 (`action = strategy.decide_action(obs, info, step); env.step(action)`)
