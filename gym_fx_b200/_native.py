@@ -85,7 +85,7 @@ INFO_DTYPES = {
 def build(force: bool = False, verbose: bool = False) -> str:
     """Compile gym_fx_b200/csrc/*.cu into gym_fx_b200/libfxenv.so with nvcc for sm_90a (works without a GPU)."""
     srcs = [os.path.join(CSRC, f) for f in ("fx_capi.cu", "fx_kernels.cu", "fx_kernels_trunc.cu", "fx_policy.cu", "fx_core.cuh",
-                                            "fx_kernels.cuh", "fx_policy.cuh", "Makefile")]
+                                            "fx_kernels.cuh", "fx_env_step.cuh", "fx_policy.cuh", "Makefile")]
     srcs.append(os.path.join(_HERE, "..", "include", "fxenv.h"))
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in srcs)
     if force or stale:

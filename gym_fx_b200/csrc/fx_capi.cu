@@ -141,6 +141,16 @@ void drop_graph(FxEnv* env) {
     if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
 }
 
+// A launch parameter in env->P is about to change: wait until no launch may still run with the old one (no cached
+// graph is destroyed while a launch of it may be running), drop the cached step-many graphs, which captured the old P,
+// and bump the epoch, so that each policy re-captures its rollout graph on its next use
+int params_changing(FxEnv* env) {
+  FX_CUDA(env, cudaDeviceSynchronize());
+  drop_graph(env);
+  env->params_epoch++;
+  return FXENV_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -610,9 +620,7 @@ int fxenv_set_bracket_audit(FxEnv* env, int32_t capacity) {
   if (capacity > 0 && records > (uint64_t)INT64_MAX / (FXENV_AU_FIELDS * sizeof(double)))
     return fail(env, FXENV_E_INVALID, "bracket audit capacity too large");
   DeviceGuard g(env->device);
-  FX_CUDA(env, cudaDeviceSynchronize());  // kernels in flight may still write the old ring
-  drop_graph(env);                        // the cached step-many graphs captured the old P
-  env->params_epoch++;                    // ... and so did each policy's rollout graph (re-captured on its next use)
+  if (const int rc = params_changing(env)) return rc;  // also: kernels in flight may still write the old ring
   cudaFree(env->P.audit); cudaFree(env->P.audit_written);
   env->P.audit = nullptr; env->P.audit_written = nullptr; env->P.audit_cap = 0;
   if (capacity == 0) return FXENV_OK;
@@ -641,9 +649,7 @@ int fxenv_set_action_repeat(FxEnv* env, int32_t repeat, uint32_t flags) {
   if (flags & ~FXENV_REPEAT_HOLD) return fail(env, FXENV_E_INVALID, "unknown action repeat flags " + std::to_string(flags));
   if (repeat == env->P.repeat && flags == env->P.repeat_flags) return FXENV_OK;
   DeviceGuard g(env->device);
-  FX_CUDA(env, cudaDeviceSynchronize());  // no cached graph is destroyed while a launch of it may be running
-  drop_graph(env);       // the cached step-many graphs captured the old P
-  env->params_epoch++;   // ... and so did each policy's rollout graph
+  if (const int rc = params_changing(env)) return rc;
   env->P.repeat = repeat;
   env->P.repeat_flags = flags;
   return FXENV_OK;
@@ -654,9 +660,7 @@ int fxenv_set_time_limit(FxEnv* env, int32_t max_steps, uint32_t flags) {
   if (max_steps < 0) return fail(env, FXENV_E_INVALID, "time limit must be >= 0 decisions, got " + std::to_string(max_steps));
   if (flags & ~FXENV_TIME_LIMIT_WINDOW) return fail(env, FXENV_E_INVALID, "unknown time limit flags " + std::to_string(flags));
   DeviceGuard g(env->device);
-  FX_CUDA(env, cudaDeviceSynchronize());  // no cached graph is destroyed, and no count zeroed, while a launch may run
-  drop_graph(env);       // the cached step-many graphs captured the old P
-  env->params_epoch++;   // ... and so did each policy's rollout graph
+  if (const int rc = params_changing(env)) return rc;  // also: no count is zeroed while a launch may run
   if ((max_steps > 0 || flags != 0u) && !env->trunc_configured) {
     // the truncation kernels' first use on this handle: their attributes, and the persistent grid's minimum over them
     // (every launch reads the grid and advances the ticket words by its own warp count)

@@ -1,4 +1,5 @@
-// fx_kernels.cuh -- device-side data layout shared by fx_kernels.cu (kernels) and fx_capi.cu (C-ABI host code).
+// fx_kernels.cuh -- device-side data layout shared by the kernels (fx_env_step.cuh, fx_kernels.cu) and fx_capi.cu
+// (C-ABI host code).
 #pragma once
 
 #include "fx_core.cuh"
@@ -153,12 +154,34 @@ cudaError_t fx_launch_rollout(const FxKernelParams& P, const void* actions, floa
 int fx_rollout_blocks(const FxKernelParams& P);
 int fx_rollout_warps(const FxKernelParams& P);  // warps of a fx_rollout_kernel launch (each draws one ticket past the last)
 int fx_order_smem_choice(const FxKernelParams& P, int force);
-// the truncation instantiations (fx_kernels_trunc.cu: fx_kernels.cu compiled with FX_KERNELS_TRUNC), picked by
-// fx_kernels.cu while fx_trunc_on(P); lean / audit / repeat as in its pick_kernel / pick_rollout
+
+// The variant key of the step / rollout kernels (DESIGN §4, "The variant key"): one bit per compile-time switch of
+// fx_step_env, chosen from the handle by fx_variant_key (fx_kernels.cu).
+enum : unsigned {
+  FX_V_FAST5 = 1u,     // the 5-feature fast path (fast_features == 5)
+  FX_V_LEAN = 2u,      // the LEAN specialisation (lean, fx_config_is_lean)
+  FX_V_RESIDENT = 4u,  // the order table resident in shared memory (order_smem)
+  FX_V_AUDIT = 8u,     // the bracket audit store (fxenv_set_bracket_audit)
+  FX_V_REPEAT = 16u,   // the action repeat (fxenv_set_action_repeat, repeat > 1)
+  FX_V_TRUNC = 32u,    // decision counts and truncation (fxenv_set_time_limit, fx_trunc_on)
+  FX_V_KEYS = 64u
+};
+enum { FX_N_STRATEGIES = FX_STRATEGY_ATR_SLTP + 1, FX_N_REWARDS = FX_REWARD_DD + 1 };
+// The keys that have kernels: LEAN needs the fast path and the audit the ATR strategy.  (FX_V_RESIDENT selects a rollout
+// kernel only: the step kernel ignores it.)
+constexpr bool fx_variant_valid(int strategy, unsigned key) {
+  return ((key & FX_V_LEAN) == 0u || (key & FX_V_FAST5) != 0u) &&
+         ((key & FX_V_AUDIT) == 0u || strategy == FX_STRATEGY_ATR_SLTP);
+}
+
 typedef void (*FxStepKernelFn)(const FxKernelParams, const void*, float*, float*, double*, uint8_t*, int, int, uint16_t*, int,
                                const FxTileSync);
 typedef void (*FxRolloutKernelFn)(const FxKernelParams, const char*, float*, int, float*, uint8_t*, const FxChunkPlan, unsigned,
                                   unsigned);
-FxStepKernelFn fx_pick_step_trunc(const FxKernelParams& P, int lean, int audit, int repeat);
-FxRolloutKernelFn fx_pick_rollout_trunc(const FxKernelParams& P, int lean, int audit, int repeat);
+struct FxEnvKernels {
+  FxStepKernelFn step;
+  FxRolloutKernelFn rollout;
+};
+// the kernels of a key with FX_V_TRUNC (fx_kernels_trunc.cu; fx_kernels.cu holds those without it)
+FxEnvKernels fx_trunc_kernels(int strategy, int reward, unsigned key);
 FxChunkPlan fx_rollout_plan(const FxKernelParams& P, int n_steps);  // the host's ticket accounting needs n_rounds

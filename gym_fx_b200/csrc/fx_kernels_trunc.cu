@@ -1,5 +1,7 @@
-// fx_kernels_trunc.cu -- the truncation instantiations of the step / rollout kernels (include/fxenv.h,
-// fxenv_set_time_limit): fx_kernels.cu with FX_KERNELS_TRUNC, its kernels inside namespace fx_trunc.  A translation unit
-// of its own, so that the kernels that run with truncation off are not touched and both halves compile in parallel.
-#define FX_KERNELS_TRUNC 1
-#include "fx_kernels.cu"
+// fx_kernels_trunc.cu -- the step / rollout kernels of fx_env_step.cuh with truncation (FX_V_TRUNC, fxenv_set_time_limit).
+// A translation unit of its own so that both halves of the kernels compile in parallel.
+#include "fx_env_step.cuh"
+
+FxEnvKernels fx_trunc_kernels(int strategy, int reward, unsigned key) {
+  return fx_variant_lookup<FX_V_TRUNC>(strategy, reward, key);
+}
