@@ -40,13 +40,7 @@
 #ifndef FX_LONG_MIN_W
 #define FX_LONG_MIN_W 384  // windows of at least this many rows use the unrolled loop
 #endif
-#ifndef FX_EMIT_INLINE
-#define FX_EMIT_INLINE __forceinline__  // the 16-byte-store row emitter inlined at its call sites
-#endif
 constexpr int kLongUnroll = FX_LONG_UNROLL;  // (a macro is not expanded inside #pragma unroll)
-#ifndef FX_EMIT_EARLY
-#define FX_EMIT_EARLY 0  // 1: emit the observation windows right after the order sweep
-#endif
 
 namespace {
 
@@ -462,9 +456,9 @@ __device__ __noinline__ void fx_emit_windows_t(const FxKernelParams& P, int lane
 // first row repeated `pad` times (feature_window_preprocessor.py:153-160,197-204) -- the first W steps of every episode.
 // What it needs of the configuration arrives BY VALUE: as a non-inlined function taking a reference to the kernel parameters
 // it read them with generic loads (a constant-bank address formed at run time), ~10 dependent round trips at the top of
-// every row.  (It is now inlined as well, FX_EMIT_INLINE.)  NOBIN: no binary pass-through feature (LEAN contract).
+// every row.  (It is now inlined as well.)  NOBIN: no binary pass-through feature (LEAN contract).
 template <bool CLIP, bool TAME, bool O16, bool PAD, bool LONG, bool NOBIN>
-__device__ FX_EMIT_INLINE void fx_emit_fast5_q(const int lane, const bool scale, const double* __restrict__ win,
+__device__ __forceinline__ void fx_emit_fast5_q(const int lane, const bool scale, const double* __restrict__ win,
                                              const double* sstat, float* __restrict__ out, uint16_t* __restrict__ o16_,
                                              const int pad, const int W, const float clipf, const int pc,
                                              const unsigned binary_mask) {
@@ -719,6 +713,64 @@ struct FxSubstep {
   bool ended;   // out: this substep ended the step (the last one, a terminating one, or the step of a terminated env)
 };
 
+// Where one env-step writes: the BASES of the caller's arrays (kernel parameters: they cost no registers).  The step's
+// element of actions / reward / terminated is at index step_row + env (step_row = step * num_envs), its observation row
+// at obs_slot_row + env (obs_slot_row = slot * num_envs), its bf16 copy (single-step kernel only) at row env of obs16.
+// Addresses are formed where they are used.
+struct FxStepOut {
+  float* obs;
+  uint16_t* obs16;
+  float* reward;
+  double* reward64;
+  uint8_t* terminated;
+  unsigned step_row, obs_slot_row;
+  int stride16;
+};
+__device__ __forceinline__ size_t fx_out_idx(const FxStepOut& o, int env) { return (size_t)o.step_row + (size_t)env; }
+__device__ __forceinline__ float* fx_obs_row(const FxKernelParams& P, const FxStepOut& o, int env) {
+  return o.obs + ((size_t)o.obs_slot_row + (size_t)env) * (size_t)P.obs_dim;
+}
+template <bool O16>
+__device__ __forceinline__ uint16_t* fx_obs_row16(const FxStepOut& o, int env) {
+  return (O16 && o.obs16) ? o.obs16 + (size_t)env * (size_t)o.stride16 : nullptr;
+}
+
+// Phase stamps of the timing build (make TIMING=1, tools/phase_timing.py): lane 0 writes stamp i of the env's FX_NSTAMP
+// (clock64, %globaltimer or a count).  In the release build the struct is empty and every call compiles to nothing.
+struct FxStamps {
+#ifdef FXENV_ENABLE_TIMING
+  long long* p;  // nullptr: FXENV_TIMING is off
+  __device__ __forceinline__ void put(int lane, int i, long long v) const { if (p && lane == 0) p[i] = v; }
+  __device__ __forceinline__ void at(int lane, int i) const { if (p && lane == 0) p[i] = clock64(); }
+  // taken only after `dep` (a loaded value) has actually arrived in a register
+  __device__ __forceinline__ void after(int lane, int i, unsigned long long dep) const {
+    if (p) { long long t; asm volatile("mov.u64 %0, %%clock64;" : "=l"(t) : "l"(dep)); if (lane == 0) p[i] = t; }
+  }
+  __device__ __forceinline__ void global(int lane, int i) const {
+    if (p && lane == 0) { long long g; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g)); p[i] = g; }
+  }
+  __device__ __forceinline__ void begin(const FxKernelParams& P, int env, int lane) {
+    p = P.timing ? P.timing + (int64_t)env * FX_NSTAMP : nullptr;
+    at(lane, 0);
+    global(lane, 10);
+  }
+  // keep two consecutive steps: the stamps move to slot = parity of the (pre-step) cursor t
+  __device__ __forceinline__ void to_slot(const FxKernelParams& P, int env, int32_t t, int lane) {
+    if (!p) return;
+    long long* nb = P.timing + ((int64_t)(t & 1) * P.cfg.num_envs + env) * FX_NSTAMP;
+    if (lane == 0) { nb[0] = p[0]; nb[10] = p[10]; }
+    p = nb;
+  }
+#else
+  __device__ __forceinline__ void put(int, int, long long) const {}
+  __device__ __forceinline__ void at(int, int) const {}
+  __device__ __forceinline__ void after(int, int, unsigned long long) const {}
+  __device__ __forceinline__ void global(int, int) const {}
+  __device__ __forceinline__ void begin(const FxKernelParams&, int, int) {}
+  __device__ __forceinline__ void to_slot(const FxKernelParams&, int, int32_t, int) {}
+#endif
+};
+
 // One env-step of one env by one warp (everything between the cross-kernel dependency wait and the release).
 // V: the variant key (FX_V_*).
 // CARRY (fx_rollout_kernel): the step leaves the env's scalar state in ws.carry and returns true if that record is valid;
@@ -736,12 +788,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
                                             const unsigned phase = 0u, const unsigned step_row = 0u, const unsigned obs_slot_row = 0u,
                                             uint16_t* __restrict__ obs16 = nullptr, const int stride16 = 0,
                                             const bool carry_in = false, FxSubstep* sub = nullptr) {
-  // `actions` / `reward` / `terminated` / `obs` are the BASES of the caller's arrays (kernel parameters: they cost no
-  // registers); this env-step's element is at index step_row + env (step_row = step * num_envs) and its observation row
-  // at obs_slot_row + env (obs_slot_row = slot * num_envs).  Addresses are formed where they are used.
-#define FX_OBS_ROW() (obs + ((size_t)obs_slot_row + (size_t)env) * (size_t)P.obs_dim)
-#define FX_OUT_IDX() ((size_t)step_row + (size_t)env)
-#define FX_OBS_ROW16() ((O16 && obs16) ? obs16 + (size_t)env * (size_t)stride16 : nullptr)  // bf16 copy (single-step kernel only)
+  const FxStepOut o{obs, obs16, reward, reward64, terminated, step_row, obs_slot_row, stride16};
   constexpr bool FAST5 = (V & FX_V_FAST5) != 0, LEAN = (V & FX_V_LEAN) != 0, RESIDENT = (V & FX_V_RESIDENT) != 0;
   constexpr bool AUDIT = (V & FX_V_AUDIT) != 0, REPEAT = (V & FX_V_REPEAT) != 0, TRUNC = (V & FX_V_TRUNC) != 0;
   constexpr bool ATR = STRATEGY == FX_STRATEGY_ATR_SLTP;
@@ -753,20 +800,8 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   const int capP = P.cap + FXO_SLACK;
   const int pair = (c.num_pairs == 1) ? 0 : env % c.num_pairs;
   const FxPairTable& tb = P.pair[pair];
-#ifdef FXENV_ENABLE_TIMING  // phase instrumentation build (make TIMING=1): tools/phase_timing.py
-  long long* tstamp = P.timing ? P.timing + (int64_t)env * FX_NSTAMP : nullptr;
-#define FX_STAMP(i) do { if (tstamp && lane == 0) tstamp[i] = clock64(); } while (0)
-  // stamp taken only after `dep` (a loaded value) has actually arrived in a register
-#define FX_STAMP_DEP(i, dep) do { if (tstamp) { long long t__; unsigned long long d__ = (unsigned long long)(dep); \
-    asm volatile("mov.u64 %0, %%clock64;" : "=l"(t__) : "l"(d__)); if (lane == 0) tstamp[i] = t__; } } while (0)
-#define FX_STAMP_GLOBAL(i) do { if (tstamp && lane == 0) { long long g__; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g__)); tstamp[i] = g__; } } while (0)
-#else
-#define FX_STAMP(i) do { } while (0)
-#define FX_STAMP_DEP(i, dep) do { } while (0)
-#define FX_STAMP_GLOBAL(i) do { } while (0)
-#endif
-  FX_STAMP(0);
-  FX_STAMP_GLOBAL(10);
+  FxStamps ts;
+  ts.begin(P, env, lane);
 
   // ---- round trip 1: one batch of independent state loads (invariants: see FxDeviceState)
   uint32_t flags;
@@ -791,9 +826,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
     nb_oh.x = cr[FX_CARRY_NBAR]; nb_oh.y = cr[FX_CARRY_NBAR + 1]; nb_lc.x = cr[FX_CARRY_NBAR + 2]; nb_lc.y = cr[FX_CARRY_NBAR + 3];
     nb_price = cr[FX_CARRY_NBAR + 4];
     if (TRUNC) dec = *fx_carry_dec(ws);
-#ifndef FX_NO_RUN_STATS
     if (lane < FX_RS_N) rsv = cr[FX_CARRY_RSTATS + lane];
-#endif
   } else {
     flags = st.flags[env];
     t = st.t[env];
@@ -809,15 +842,13 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
     nb_oh = nb2[0]; nb_lc = nb2[1];
     nb_price = st.nbar[(int64_t)env * 6 + 4];
     if (TRUNC) dec = P.ep_steps[env];
-#ifndef FX_NO_RUN_STATS
     if (lane < FX_RS_N) rsv = st.rstats[(int64_t)env * FX_RS_N + lane];  // DrawDown / TradeAnalyzer / SQN state
-#endif
   }
   e.value = e.equity;
   int action_raw_i = 0;
   float action_raw_f = 0.0f;
-  if (!LEAN && c.action_mode == FX_ACTION_CONTINUOUS) action_raw_f = reinterpret_cast<const float*>(actions)[FX_OUT_IDX()];
-  else action_raw_i = reinterpret_cast<const int32_t*>(actions)[FX_OUT_IDX()];
+  if (!LEAN && c.action_mode == FX_ACTION_CONTINUOUS) action_raw_f = reinterpret_cast<const float*>(actions)[fx_out_idx(o, env)];
+  else action_raw_i = reinterpret_cast<const int32_t*>(actions)[fx_out_idx(o, env)];
   // the first 32 orders of the table sit at an address that only depends on the env: they travel with the state
   // (RESIDENT: the table is read from the warp's shared memory instead, no prefetch)
   const int64_t obase = (int64_t)env * capP;
@@ -828,20 +859,10 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   uint32_t pm0 = 0u;
   double pp0 = 0.0, pp1 = 0.0, psz = 0.0;
   if (!RESIDENT) { pm0 = gmeta[lane]; pp0 = gp0[lane]; pp1 = gp1[lane]; psz = gsz[lane]; }
-#ifndef FX_NO_RUN_STATS
   const FxRunStatsWarp rs{rsv, lane};
-#else   // A/B timing builds only
-  const FxRunStatsNone rs;
-#endif
 
-#ifdef FXENV_ENABLE_TIMING
-  if (tstamp) {  // keep two consecutive steps: slot = parity of the (pre-step) cursor
-    long long* nb = P.timing + ((int64_t)(t & 1) * c.num_envs + env) * FX_NSTAMP;
-    if (lane == 0) { nb[0] = tstamp[0]; nb[10] = tstamp[10]; }
-    tstamp = nb;
-  }
-#endif
-  FX_STAMP_DEP(2, (unsigned long long)flags + (unsigned long long)t + (unsigned long long)start + (unsigned long long)total_bars);
+  ts.to_slot(P, env, t, lane);
+  ts.after(lane, 2, (unsigned long long)flags + (unsigned long long)t + (unsigned long long)start + (unsigned long long)total_bars);
 
   // ---- terminated envs: the reference answers (obs, 0.0, True) without touching plugins (app/env.py:137-138);
   //      with auto_reset (build-side extension) the env restarts its episode window instead.  A truncated env is
@@ -867,10 +888,10 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       e.price = tb.candles[(start + t) * (int64_t)C + 3];
     }
     if (lane == 0) {
-      reward[FX_OUT_IDX()] = 0.0f;
-      if (reward64) reward64[FX_OUT_IDX()] = 0.0;
-      terminated[FX_OUT_IDX()] = c.auto_reset ? 0 : ((TRUNC && !(flags & FX_FLAG_TERMINATED)) ? FXENV_DONE_TRUNCATED : 1);
-      fx_write_scalars<LEAN>(P, e, total_bars, tb.candles[(start + e.bar_index - 1) * (int64_t)C + c.price_col], FX_OBS_ROW(), FX_OBS_ROW16());
+      o.reward[fx_out_idx(o, env)] = 0.0f;
+      if (o.reward64) o.reward64[fx_out_idx(o, env)] = 0.0;
+      o.terminated[fx_out_idx(o, env)] = c.auto_reset ? 0 : ((TRUNC && !(flags & FX_FLAG_TERMINATED)) ? FXENV_DONE_TRUNCATED : 1);
+      fx_write_scalars<LEAN>(P, e, total_bars, tb.candles[(start + e.bar_index - 1) * (int64_t)C + c.price_col], fx_obs_row(P, o, env), fx_obs_row16<O16>(o, env));
     }
     {
       const int s = e.bar_index;
@@ -880,7 +901,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       const int shift = fx_window_issue(tb, C, start, left, s - left, lane, ws);
       const bool scale = fx_prepare_stats(P, tb, env, lane, s, start, ws.stat);
       fx_window_wait(ws, phase);
-      fx_emit_windows<FAST5, O16, LEAN>(P, lane, s, scale, ws.win + shift, ws.stat, FX_OBS_ROW(), FX_OBS_ROW16());
+      fx_emit_windows<FAST5, O16, LEAN>(P, lane, s, scale, ws.win + shift, ws.stat, fx_obs_row(P, o, env), fx_obs_row16<O16>(o, env));
     }
     if (REPEAT) sub->ended = true;  // rule 1 of the repeat: a terminated env runs this one substep
     return false;  // (the carry record does not follow resets / ended episodes: the next step reloads the arrays)
@@ -924,39 +945,8 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
     win_shift = fx_window_issue(tb, C, start, win_left, s_obs - win_left, lane, ws,
                                 table_stats ? tb.stats + (start + t) * (int64_t)c.n_features * 2 : nullptr, c.n_features);
 
-  FX_STAMP_DEP(1, __double_as_longlong(b.o) + __double_as_longlong(b.c));  // the new bar has arrived
+  ts.after(lane, 1, __double_as_longlong(b.o) + __double_as_longlong(b.c));  // the new bar has arrived
 
-  // ---- observation windows (app/env.py:160 -> preprocessor.make_observation) from the staged copy.  They depend on
-  // the bar cursor only (not on what the broker / strategy did); emitting them right after the order sweep
-  // (FX_EMIT_EARLY, so that the row's stores drain under the strategy / reward / write-back) was measured and is slower.
-  // Running z-score statistics while the history window is still growing (or expanding_zscore): warm-up path, one
-  // extra round trip here instead of registers held across the broker pass.
-#define FX_EMIT_OBSERVATION()                                                                              \
-  do {                                                                                                     \
-    if (REPEAT && emit && !last_sub && !(dbg & 1)) {                                                       \
-      __syncwarp();                                                                                        \
-      win_shift = fx_window_issue(tb, C, start, win_left, s_obs - win_left, lane, ws,                      \
-                                  table_stats ? tb.stats + (start + t) * (int64_t)c.n_features * 2 : nullptr, c.n_features); \
-    }                                                                                                      \
-    if (lane < c.n_features && (welford_live || ((!REPEAT || emit) && scale && !table_stats))) {           \
-      const int64_t wi = ((int64_t)env * FXENV_MAX_FEATURES + lane) * 2;                                   \
-      double wf_m = st.welford[wi], wf_m2 = st.welford[wi + 1];                                            \
-      if (welford_live) {                                                                                  \
-        fx_welford_step(wf_m, wf_m2, row[c.feature_cols[lane]], t + 1);                                    \
-        st.welford[wi] = wf_m; st.welford[wi + 1] = wf_m2;                                                 \
-      }                                                                                                    \
-      if ((!REPEAT || emit) && scale && !table_stats) {                                                    \
-        double st_m, st_r;                                                                                 \
-        fx_welford_to_stats(wf_m, wf_m2, hn, st_m, st_r);                                                  \
-        ws.stat[2 * lane] = st_m; ws.stat[2 * lane + 1] = st_r;                                            \
-      }                                                                                                    \
-    }                                                                                                      \
-    __syncwarp();                                                                                          \
-    if ((!REPEAT || emit) && !(dbg & 1)) {                                                                 \
-      fx_window_wait(ws, phase);                                                                           \
-      fx_emit_windows<FAST5, O16, LEAN>(P, lane, s_obs, scale, ws.win + win_shift, ws.stat, FX_OBS_ROW(), FX_OBS_ROW16()); \
-    }                                                                                                      \
-  } while (0)
 
   double nbar_next = 0.0;
   if (!(dbg & 2)) {
@@ -979,14 +969,12 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
           first_sub = n;    // nothing left to accept in the pass below
           reload0 = true;   // the prefetched chunk may be stale
         }
-        FX_STAMP(3);
+        ts.at(lane, 3);
         // ---- BackBroker.next(): ONE streaming pass over the table, 32 entries (one per lane) at a time, in registers:
         //      activate queued children -> trigger test (ballot) -> execute the hits in FIFO order (fields broadcast by
         //      shuffle from the owning lane) -> stable compaction + write-back of what changed.
         int w = 0;
-#ifdef FXENV_ENABLE_TIMING
-        int n_fills = 0;
-#endif
+        int n_fills = 0;  // (timing build only)
         uint32_t carry = 0u;  // operation for the first entry of the next chunk (bracket pair of a parent in lane 31)
         if (!RESIDENT && reload0 && lane < n) { pm0 = gmeta[lane]; pp0 = gp0[lane]; pp1 = gp1[lane]; psz = gsz[lane]; }
         for (int k0 = 0; k0 < n; k0 += 32) {
@@ -1016,15 +1004,9 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
             const uint32_t kind = bm & FXO_KIND_MASK;
             if (kind == FXO_PAIR && !(bm & FXO_ACTIVE)) continue;
             // Completed or Margin: either way the entry leaves the table (a PAIR: sibling / group cancelled)
-#ifdef FX_RS_NO_TRADE   // A/B timing builds only
-            const bool margin = fx_execute<LEAN>(c, e, __shfl_sync(FX_FULL, sz, l), __shfl_sync(FX_FULL, px_lane, l), FxRunStatsNone());
-#else
             const bool margin = fx_execute<LEAN>(c, e, __shfl_sync(FX_FULL, sz, l), __shfl_sync(FX_FULL, px_lane, l), rs);
-#endif
             any_fill = true;
-#ifdef FXENV_ENABLE_TIMING
             n_fills++;
-#endif
             if (lane == l) m |= FXO_DEAD;
             if (kind == FXO_PARENT) {
               const uint32_t op = margin ? FX_OP_KILL : ((!LEAN && c.children_same_bar) ? FX_OP_ACTIVATE : FX_OP_ACTIVATE_NEXT);
@@ -1042,14 +1024,11 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
           w += __popc(km);
         }
         n_live = w;
-#ifdef FXENV_ENABLE_TIMING
-        if (tstamp && lane == 0) tstamp[4] = ((long long)n << 32) | (long long)n_fills;  // debug: table size, fills
-#endif
+        ts.put(lane, 4, ((long long)n << 32) | (long long)n_fills);  // debug: table size, fills
       }
       fx_mark_to_market<LEAN>(c, e, b.c);
       // DrawDown analyzer: one notify_fund + next per bar.  With no position and no execution the value is the one of
       // the previous bar and nothing can change.
-#ifndef FX_NO_RUN_STATS
       if (any_fill || e.psize != 0.0) {
         // fx_rs_drawdown in the lane layout: ONE broadcast (the peak), then lanes 0 / 1 / 2 each test their own field;
         // the percent needs its division only when it can set a new maximum.  The record goes back to memory only when
@@ -1065,17 +1044,13 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
         if (up) rsv = cand;
         if (any_fill || __any_sync(FX_FULL, up)) { if (lane < FX_RS_N) st.rstats[(int64_t)env * FX_RS_N + lane] = rsv; }
       }
-#endif
     }
-    FX_STAMP(5);  // broker pass done, marked to market
+    ts.at(lane, 5);  // broker pass done, marked to market
     // candle of the next call (lanes 0..4): requested now, stored at the end of the env-step
     if (lane < 5) {
       const int tn = (t + 1 < total_bars) ? t + 1 : total_bars - 1;
       nbar_next = tb.candles[(start + tn) * (int64_t)C + (lane < 4 ? lane : c.price_col)];
     }
-#if FX_EMIT_EARLY
-    FX_EMIT_OBSERVATION();
-#endif
 
     double r;
     int n_final = n_live, n_acc_new = n_live;
@@ -1137,7 +1112,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       e.price = b.c;
       n_acc_new = n_acc; sub_need_new = sub_need;  // nothing was processed
     }
-    FX_STAMP(6);  // strategy + publish
+    ts.at(lane, 6);  // strategy + publish
 
     // ---- reward plugin (app/env.py:148-155)
     if (REWARD == FX_REWARD_PNL) {
@@ -1187,7 +1162,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       dec += 1;
       if (!term && !trunc && P.max_steps > 0 && dec >= P.max_steps) { e.flags |= FX_FLAG_TRUNCATED; trunc = true; }
     }
-    FX_STAMP(7);  // reward
+    ts.at(lane, 7);  // reward
 
     // ---- write back (lane 0): always-changing columns, then the ones a fill touched
     if (lane == 0) {
@@ -1203,10 +1178,10 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       if (sub_need_new != sub_need) st.sub_need[env] = sub_need_new;
       if (TRUNC) P.ep_steps[env] = dec;
       if (!REPEAT || emit) {
-        reward[FX_OUT_IDX()] = (float)r;
-        if (reward64) reward64[FX_OUT_IDX()] = r;
-        terminated[FX_OUT_IDX()] = term ? 1 : ((TRUNC && trunc) ? FXENV_DONE_TRUNCATED : 0);
-        fx_write_scalars<LEAN>(P, e, total_bars, last_price, FX_OBS_ROW(), FX_OBS_ROW16());
+        o.reward[fx_out_idx(o, env)] = (float)r;
+        if (o.reward64) o.reward64[fx_out_idx(o, env)] = r;
+        o.terminated[fx_out_idx(o, env)] = term ? 1 : ((TRUNC && trunc) ? FXENV_DONE_TRUNCATED : 0);
+        fx_write_scalars<LEAN>(P, e, total_bars, last_price, fx_obs_row(P, o, env), fx_obs_row16<O16>(o, env));
       }
       if (CARRY) {  // what the env's next step starts from, should this warp run it (the arrays above stay authoritative)
         double* __restrict__ cr = ws.carry;
@@ -1225,33 +1200,46 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       }
     }
   } else {  // timing experiment only (FXENV_DEBUG & 2): cursor only
-    if (lane == 0) { st.t[env] = t; st.flags[env] = flags; st.bar_index[env] = t + 1; reward[FX_OUT_IDX()] = 0.f; terminated[FX_OUT_IDX()] = 0; }
-#if FX_EMIT_EARLY
-    FX_EMIT_OBSERVATION();
-#endif
+    if (lane == 0) { st.t[env] = t; st.flags[env] = flags; st.bar_index[env] = t + 1; o.reward[fx_out_idx(o, env)] = 0.f; o.terminated[fx_out_idx(o, env)] = 0; }
   }
-  FX_STAMP(8);  // scalars written back
+  ts.at(lane, 8);  // scalars written back
 
-#if !FX_EMIT_EARLY
-  FX_EMIT_OBSERVATION();
-#endif
+  // ---- observation windows (app/env.py:160 -> preprocessor.make_observation) from the staged copy.  They depend on
+  // the bar cursor only (not on what the broker / strategy did); emitting them right after the order sweep (so that
+  // the row's stores drain under the strategy / reward / write-back) was measured and is slower.
+  // Running z-score statistics while the history window is still growing (or expanding_zscore): warm-up path, one
+  // extra round trip here instead of registers held across the broker pass.
+  if (REPEAT && emit && !last_sub && !(dbg & 1)) {
+    __syncwarp();
+    win_shift = fx_window_issue(tb, C, start, win_left, s_obs - win_left, lane, ws,
+                                table_stats ? tb.stats + (start + t) * (int64_t)c.n_features * 2 : nullptr, c.n_features);
+  }
+  if (lane < c.n_features && (welford_live || ((!REPEAT || emit) && scale && !table_stats))) {
+    const int64_t wi = ((int64_t)env * FXENV_MAX_FEATURES + lane) * 2;
+    double wf_m = st.welford[wi], wf_m2 = st.welford[wi + 1];
+    if (welford_live) {
+      fx_welford_step(wf_m, wf_m2, row[c.feature_cols[lane]], t + 1);
+      st.welford[wi] = wf_m; st.welford[wi + 1] = wf_m2;
+    }
+    if ((!REPEAT || emit) && scale && !table_stats) {
+      double st_m, st_r;
+      fx_welford_to_stats(wf_m, wf_m2, hn, st_m, st_r);
+      ws.stat[2 * lane] = st_m; ws.stat[2 * lane + 1] = st_r;
+    }
+  }
+  __syncwarp();
+  if ((!REPEAT || emit) && !(dbg & 1)) {
+    fx_window_wait(ws, phase);
+    fx_emit_windows<FAST5, O16, LEAN>(P, lane, s_obs, scale, ws.win + win_shift, ws.stat, fx_obs_row(P, o, env), fx_obs_row16<O16>(o, env));
+  }
   if (lane < 5 && !(dbg & 2)) st.nbar[(int64_t)env * 6 + lane] = nbar_next;
   if (CARRY) {
     if (lane < 5) ws.carry[FX_CARRY_NBAR + lane] = nbar_next;
-#ifndef FX_NO_RUN_STATS
     if (lane < FX_RS_N) ws.carry[FX_CARRY_RSTATS + lane] = rsv;
-#endif
   }
   if (REPEAT) sub->ended = emit;
-  FX_STAMP(9);
-  FX_STAMP_GLOBAL(11);
-#undef FX_EMIT_OBSERVATION
-#undef FX_OBS_ROW
-#undef FX_OBS_ROW16
-#undef FX_OUT_IDX
-#undef FX_STAMP
-#undef FX_STAMP_DEP
-#undef FX_STAMP_GLOBAL
+  ts.at(lane, 9);
+  ts.global(lane, 11);
   return CARRY && !(dbg & 2);
 }
 
@@ -1283,11 +1271,7 @@ __device__ __forceinline__ int fx_ld_acquire(const int32_t* p) {
   return v;
 }
 __device__ __forceinline__ void fx_st_release(int32_t* p, int v) {
-#ifdef FX_UNSAFE_NO_FENCE  // TIMING EXPERIMENT ONLY (results are racy): what would a fence-free hand-over be worth?
-  asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" :: "l"(p), "r"(v) : "memory");
-#else
   asm volatile("st.release.gpu.global.s32 [%0], %1;" :: "l"(p), "r"(v) : "memory");
-#endif
 }
 
 // The single-step kernel: one warp per env, one env per CTA.  Launched with the programmatic-dependent-launch attribute:
