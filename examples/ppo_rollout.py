@@ -13,6 +13,7 @@ minibatch and advantages are normalised with global statistics (gym_fx_b200.lear
     python examples/ppo_rollout.py --envs 4096 --episode-bars 500 --holdout-frac 0.2 --eval-rollouts 2
     python examples/ppo_rollout.py --envs 4096 --action-repeat 5 --repeat-mode hold
     python examples/ppo_rollout.py --hidden 64
+    python examples/ppo_rollout.py --randomize-costs 1e-4,3e-4
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 examples/ppo_rollout.py --envs 4096
 
 --action-space continuous trains a Gaussian actor on the Box(-1, 1) action (thresholded to hold / long / short by the
@@ -32,6 +33,9 @@ last observation instead of treating the cut as the end of the market.  Before t
 staggered: in 8 groups, each reset after a different number of hold decisions, so that their cuts spread over the run
 instead of falling on the same step.  terminated_frac / truncated_frac: the share of the last rollout's steps with each
 code.
+--randomize-costs COMM_MAX,SLIP_MAX draws each env's commission and slippage uniformly from [0, COMM_MAX] and [0, SLIP_MAX]
+before every rollout (VecFxEnv.set_env_params: the values change in place, the rollout graph stays), so that the policy
+does not fit one cost model.
 Prints one JSON line: env-steps/s (decisions) of the rollout phase (policy in the loop) and of the whole train loop, and
 bars/s of the rollout phase as an upper bound (decisions x K: a step that ends an episode runs fewer bars).
 """
@@ -43,6 +47,7 @@ import os
 import sys
 import time
 
+import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -73,8 +78,18 @@ def main():
                     help="time limit: an episode is truncated after this many decisions (0: none)")
     ap.add_argument("--truncate-window", action="store_true",
                     help="the end of an episode window is a truncation (bootstrapped), not a termination")
+    ap.add_argument("--randomize-costs", default=None, metavar="COMM_MAX,SLIP_MAX",
+                    help="draw each env's commission and slippage uniformly from [0, max] before every rollout")
     args = ap.parse_args()
     continuous = args.action_space == "continuous"
+    cost_max = None
+    if args.randomize_costs is not None:
+        try:
+            cost_max = tuple(float(x) for x in args.randomize_costs.split(","))
+        except ValueError:
+            cost_max = ()
+        if len(cost_max) != 2 or not (cost_max[0] >= 0.0 and 0.0 <= cost_max[1] < 1.0):
+            ap.error("--randomize-costs takes COMM_MAX,SLIP_MAX with COMM_MAX >= 0 and 0 <= SLIP_MAX < 1")
     if not 0.0 <= args.holdout_frac < 1.0:
         ap.error("--holdout-frac must be in [0, 1)")
     if args.holdout_frac > 0.0 and args.episode_bars <= 0:
@@ -153,7 +168,13 @@ def main():
 
     t_roll = t_upd = 0.0
     stats = {}
+    cost_rng = np.random.default_rng(0xC057 + rank) if cost_max else None
+    if cost_max:
+        desc += f", commission ~ U[0, {cost_max[0]:g}] and slippage ~ U[0, {cost_max[1]:g}] per env and rollout"
     for it in range(args.updates):
+        if cost_max:   # per-iteration cost randomisation: the table changes in place (outside the timed rollout)
+            env.set_env_params(commission=cost_rng.uniform(0.0, cost_max[0], N),
+                               slippage=cost_rng.uniform(0.0, cost_max[1], N))
         torch.cuda.synchronize(dev)
         t0 = time.perf_counter()
         buf = env.rollout(policy, H, buffers=buf, seed=1000 * rank + it)
@@ -216,7 +237,7 @@ def main():
             "policy": f"MLP({D},{args.hidden},{args.hidden}) actor-critic ({args.action_space} actions), fused wgmma kernel in the rollout, "
                       "torch (tf32) in the update",
             "hidden": args.hidden, "rollout_env_steps_per_s": steps / max(t_roll, 1e-9), "rollout_us_per_step": t_roll / (H * n_it) * 1e6,
-            "action_repeat": K, "repeat_mode": args.repeat_mode,
+            "action_repeat": K, "repeat_mode": args.repeat_mode, "randomize_costs": list(cost_max) if cost_max else None,
             "rollout_bars_per_s_upper_bound": steps * K / max(t_roll, 1e-9),
             "train_env_steps_per_s": steps / max(t_roll + t_upd, 1e-9), "update_s": t_upd / n_it, **stats}), flush=True)
     env.close()

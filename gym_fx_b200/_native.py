@@ -32,7 +32,7 @@ EXPORTS = [
     "fxenv_policy_create", "fxenv_policy_set_weights", "fxenv_policy_destroy", "fxenv_rollout", "fxenv_policy_sync_timeouts",
     "fxenv_rollout_ex", "fxenv_policy_peek", "fxenv_set_reset_starts", "fxenv_get_episode_info",
     "fxenv_set_bracket_audit", "fxenv_get_bracket_audit", "fxenv_set_action_repeat", "fxenv_policy_create_ex",
-    "fxenv_set_time_limit",
+    "fxenv_set_time_limit", "fxenv_set_env_params",
 ]
 
 ROLLOUT_GREEDY = 1  # FXENV_ROLLOUT_GREEDY
@@ -41,6 +41,9 @@ MAX_REPEAT, REPEAT_HOLD = 256, 1  # FXENV_MAX_REPEAT, FXENV_REPEAT_HOLD
 POLICY_WIDTHS = (64, 128, 256, 512)  # the hidden widths fxenv_policy_create_ex accepts
 FLAG_TRUNCATED, TIME_LIMIT_WINDOW = 64, 1  # FX_FLAG_TRUNCATED, FXENV_TIME_LIMIT_WINDOW
 DONE_TERMINATED, DONE_TRUNCATED = 1, 2  # FXENV_DONE_* codes of the terminated / done outputs while truncation is on
+# FXENV_ENV_PARAMS and the FXENV_PARAM_* columns of a per-env parameter row (fxenv_set_env_params)
+ENV_PARAMS = 7
+PARAM_COMMISSION, PARAM_LEVERAGE, PARAM_SLIPPAGE, PARAM_SL_PIPS, PARAM_TP_PIPS, PARAM_K_SL, PARAM_K_TP = range(7)
 
 
 class FxEnvError(RuntimeError):
@@ -84,12 +87,13 @@ INFO_DTYPES = {
 
 def build(force: bool = False, verbose: bool = False) -> str:
     """Compile gym_fx_b200/csrc/*.cu into gym_fx_b200/libfxenv.so with nvcc for sm_90a (works without a GPU)."""
-    srcs = [os.path.join(CSRC, f) for f in ("fx_capi.cu", "fx_kernels.cu", "fx_kernels_trunc.cu", "fx_policy.cu", "fx_core.cuh",
+    srcs = [os.path.join(CSRC, f) for f in ("fx_capi.cu", "fx_kernels.cu", "fx_kernels_trunc.cu", "fx_kernels_params.cu",
+                                            "fx_kernels_params_trunc.cu", "fx_policy.cu", "fx_core.cuh",
                                             "fx_kernels.cuh", "fx_env_step.cuh", "fx_policy.cuh", "Makefile")]
     srcs.append(os.path.join(_HERE, "..", "include", "fxenv.h"))
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in srcs)
     if force or stale:
-        cmd = ["make", "-j4", "-C", CSRC] + (["-B"] if force else [])  # the sources compile in parallel
+        cmd = ["make", "-j6", "-C", CSRC] + (["-B"] if force else [])  # the sources compile in parallel
         out = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if verbose or out.returncode != 0:
             print(out.stdout)
@@ -148,6 +152,7 @@ def load():
     L.fxenv_get_bracket_audit.argtypes = [vp, C.POINTER(FxAuditPtrs)]
     L.fxenv_set_action_repeat.argtypes = [vp, C.c_int32, C.c_uint32]
     L.fxenv_set_time_limit.argtypes = [vp, C.c_int32, C.c_uint32]
+    L.fxenv_set_env_params.argtypes = [vp, vp]
     if L.fxenv_abi_version() != 2:
         raise FxEnvError("libfxenv.so ABI version mismatch")
     _lib = L

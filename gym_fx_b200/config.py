@@ -312,6 +312,51 @@ def lower_config(
     return c
 
 
+# The columns of a per-env parameter row (include/fxenv.h FXENV_PARAM_*) and the FxConfig field each one replaces
+ENV_PARAM_FIELDS = ("commission", "leverage", "slippage", "sl_pips", "tp_pips", "k_sl", "k_tp")
+_ENV_PARAM_CFG = ("commission", "leverage", "slippage_perc", "sl_pips", "tp_pips", "k_sl", "k_tp")
+
+
+def env_params_table(cfg: FxConfig, **fields) -> "np.ndarray":
+    """The float64 [num_envs, 7] table of fxenv_set_env_params (VecFxEnv.set_env_params).  Each keyword of
+    ENV_PARAM_FIELDS is None (the config's value for every env), a scalar (every env) or num_envs values (a sequence, numpy
+    array or tensor).  Raises TypeError for an unknown field or a non-numeric value, ValueError for a wrong length, a value
+    that is not finite, leverage <= 0 or slippage outside [0, 1) (the rules fxenv_create applies to the config)."""
+    import numpy as np
+
+    unknown = sorted(set(fields) - set(ENV_PARAM_FIELDS))
+    if unknown:
+        raise TypeError(f"unknown env parameter(s) {unknown}; expected some of {ENV_PARAM_FIELDS}")
+    n = int(cfg.num_envs)
+    table = np.empty((n, len(ENV_PARAM_FIELDS)), np.float64)
+    for j, (name, cname) in enumerate(zip(ENV_PARAM_FIELDS, _ENV_PARAM_CFG)):
+        v = fields.get(name)
+        if v is None:
+            table[:, j] = getattr(cfg, cname)
+            continue
+        if hasattr(v, "detach"):  # torch tensor, on any device
+            v = v.detach().cpu().numpy()
+        a = np.asarray(v)
+        if a.dtype.kind not in "iuf":
+            raise TypeError(f"{name} must be numeric, got {a.dtype} ({v!r:.60})")
+        if a.ndim == 0 or a.shape == (n,):
+            table[:, j] = a.astype(np.float64)
+        else:
+            raise ValueError(f"{name} must be a scalar or {n} values (one per env), got shape {a.shape}")
+    for j, name in enumerate(ENV_PARAM_FIELDS):
+        col = table[:, j]
+        bad = ~np.isfinite(col)
+        if name == "leverage":
+            bad |= ~(col > 0.0)
+        elif name == "slippage":
+            bad |= ~((col >= 0.0) & (col < 1.0))
+        if bad.any():
+            i = int(np.flatnonzero(bad)[0])
+            rule = {"leverage": "finite and > 0", "slippage": "in [0, 1)"}.get(name, "finite")
+            raise ValueError(f"env {i}: {name} = {col[i]!r} must be {rule}")
+    return table
+
+
 def obs_dim(cfg: FxConfig) -> int:
     """Flat observation width (SURVEY A.2): features W*F | prices W | returns W | 4 agent scalars."""
     W = cfg.window_size

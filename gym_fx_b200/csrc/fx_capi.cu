@@ -1,6 +1,7 @@
 // fx_capi.cu -- the C-ABI of libfxenv.so (include/fxenv.h): handle management, device memory, kernel launches.
 // No torch types, no exceptions across the boundary; every entry point returns a status code.
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -69,6 +70,12 @@ struct FxEnv {
   // graph captured the old P by value (FxPolicy::cached)
   uint64_t params_epoch = 0;
   bool trunc_configured = false;   // fx_configure_trunc_kernels has run (fxenv_set_time_limit)
+  // per-env parameters (fxenv_set_env_params): the host copy of the table while it is on (the LEAN choice is made on its
+  // values).  The device table lives behind the sequence words in the allocation of P.seq, at params_off (0: not yet
+  // allocated); P.env_params_off is params_off while the table is on and 0 while it is off.
+  std::vector<double> params_host;
+  uint32_t params_off = 0;
+  bool params_configured = false;  // fx_configure_params_kernels has run (the truncation half too once trunc_configured)
 };
 
 namespace {
@@ -148,6 +155,24 @@ int params_changing(FxEnv* env) {
   FX_CUDA(env, cudaDeviceSynchronize());
   drop_graph(env);
   env->params_epoch++;
+  return FXENV_OK;
+}
+
+// Whether the handle runs the LEAN kernels (fx_config_is_lean): decided once every candle table is loaded, on the costs
+// of the per-env table `rows` ([N][FXENV_ENV_PARAMS] host copy) if one is on
+int lean_choice(const FxEnv* env, const double* rows) {
+  for (int p = 0; p < env->P.cfg.num_pairs; p++)
+    if (!env->loaded[p]) return 0;
+  if (getenv("FXENV_NO_LEAN")) return 0;
+  return fx_config_is_lean(env->P, rows) ? 1 : 0;
+}
+
+// The check_submitted cash bound each env keeps for the orders its last strategy call submitted (FxDeviceState::sub_need)
+// was computed with the costs of that call.  After the costs may have changed (a per-env table set, changed or turned
+// off, or a snapshot restored on a handle that has had one), +inf makes the next env-step run the exact check instead.
+int invalidate_cash_bounds(FxEnv* env) {
+  const std::vector<double> inf((size_t)env->P.cfg.num_envs, INFINITY);
+  FX_CUDA(env, cudaMemcpy(env->P.st.sub_need, inf.data(), inf.size() * sizeof(double), cudaMemcpyHostToDevice));
   return FXENV_OK;
 }
 
@@ -329,9 +354,7 @@ int fxenv_load_candles(FxEnv* env, int pair_id, const double* candles_host, int6
   env->tame[pair_id] = tame;
   env->P.tame_data = 1;
   for (int p = 0; p < c.num_pairs; p++) if (env->loaded[p] && !env->tame[p]) env->P.tame_data = 0;
-  bool all_loaded = true;
-  for (int p = 0; p < c.num_pairs; p++) all_loaded = all_loaded && env->loaded[p];
-  env->P.lean = (all_loaded && !getenv("FXENV_NO_LEAN") && fx_config_is_lean(env->P)) ? 1 : 0;
+  env->P.lean = lean_choice(env, env->P.env_params_off ? env->params_host.data() : nullptr);
   return FXENV_OK;
 }
 
@@ -565,6 +588,9 @@ int fxenv_set_state(FxEnv* env, const void* buf_host, int64_t nbytes) {
   DeviceGuard g(env->device);
   FX_CUDA(env, cudaDeviceSynchronize());
   FX_CUDA(env, cudaMemcpy(env->slab, static_cast<const char*>(buf_host) + sizeof got, env->slab_bytes, cudaMemcpyHostToDevice));
+  if (env->params_configured) {  // the blob's cash bounds may stem from other per-env costs
+    if (const int rc = invalidate_cash_bounds(env)) return rc;
+  }
   env->was_reset = true;
   env->first_reset = false;
   return FXENV_OK;
@@ -665,6 +691,7 @@ int fxenv_set_time_limit(FxEnv* env, int32_t max_steps, uint32_t flags) {
     // the truncation kernels' first use on this handle: their attributes, and the persistent grid's minimum over them
     // (every launch reads the grid and advances the ticket words by its own warp count)
     FX_CUDA(env, fx_configure_trunc_kernels(env->P));
+    if (env->params_configured) FX_CUDA(env, fx_configure_params_kernels(env->P, FX_V_TRUNC));
     env->trunc_configured = true;
   }
   env->P.max_steps = max_steps;
@@ -673,6 +700,69 @@ int fxenv_set_time_limit(FxEnv* env, int32_t max_steps, uint32_t flags) {
   FX_CUDA(env, cudaMemset(env->P.ep_steps, 0, (size_t)env->P.cfg.num_envs * sizeof(int32_t)));
   FX_CUDA(env, cudaDeviceSynchronize());
   return FXENV_OK;
+}
+
+int fxenv_set_env_params(FxEnv* env, const double* params_host) {
+  if (!env) return FXENV_E_INVALID;
+  const size_t N = (size_t)env->P.cfg.num_envs;
+  if (params_host) {  // every row first: a bad one leaves the table in force as it was
+    static const char* const names[FXENV_ENV_PARAMS] = {"commission", "leverage", "slippage", "sl_pips", "tp_pips", "k_sl", "k_tp"};
+    for (size_t i = 0; i < N; i++) {
+      const double* r = params_host + i * FXENV_ENV_PARAMS;
+      char buf[160];
+      for (int j = 0; j < FXENV_ENV_PARAMS; j++)
+        if (!isfinite(r[j])) {
+          snprintf(buf, sizeof buf, "env params: env %zu: %s is %g; every field must be finite", i, names[j], r[j]);
+          return fail(env, FXENV_E_INVALID, buf);
+        }
+      if (!(r[FXENV_PARAM_LEVERAGE] > 0.0)) {
+        snprintf(buf, sizeof buf, "env params: env %zu: leverage is %g; it must be > 0", i, r[FXENV_PARAM_LEVERAGE]);
+        return fail(env, FXENV_E_INVALID, buf);
+      }
+      if (!(r[FXENV_PARAM_SLIPPAGE] >= 0.0 && r[FXENV_PARAM_SLIPPAGE] < 1.0)) {
+        snprintf(buf, sizeof buf, "env params: env %zu: slippage is %g; it must be in [0, 1)", i, r[FXENV_PARAM_SLIPPAGE]);
+        return fail(env, FXENV_E_INVALID, buf);
+      }
+    }
+  }
+  DeviceGuard g(env->device);
+  const bool was_on = env->P.env_params_off != 0u;
+  // the kernel choice under the new table: a change of it (or of on / off) drops the graphs captured with the old one
+  const int lean = lean_choice(env, params_host);
+  if (was_on != (params_host != nullptr) || lean != env->P.lean) {
+    if (const int rc = params_changing(env)) return rc;
+  } else {
+    FX_CUDA(env, cudaDeviceSynchronize());  // no launch may still read the old values
+  }
+  if (params_host) {
+    if (!env->params_configured) {
+      // the per-env parameter kernels' first use on this handle: their attributes and the persistent grid's minimum
+      FX_CUDA(env, fx_configure_params_kernels(env->P, 0u));
+      if (env->trunc_configured) FX_CUDA(env, fx_configure_params_kernels(env->P, FX_V_TRUNC));
+      env->params_configured = true;
+    }
+    if (!env->params_off) {
+      // the first table: the allocation of the sequence words grows by the table (fx_env_params); the words move along
+      // (no launch is running: params_changing synchronised)
+      const size_t words = (N + 1) * sizeof(int32_t), off = (words + 255) & ~(size_t)255;
+      int32_t* seq = nullptr;
+      FX_CUDA(env, cudaMalloc(&seq, off + N * FXENV_ENV_PARAMS * sizeof(double)));
+      const cudaError_t e = cudaMemcpy(seq, env->P.seq, words, cudaMemcpyDeviceToDevice);
+      if (e != cudaSuccess) { cudaFree(seq); return cuda_fail(env, e, "cudaMemcpy(seq)"); }
+      cudaFree(env->P.seq);
+      env->P.seq = seq;
+      env->params_off = (uint32_t)off;
+    }
+    env->P.env_params_off = env->params_off;
+    FX_CUDA(env, cudaMemcpy(const_cast<double*>(fx_env_params(env->P)), params_host, N * FXENV_ENV_PARAMS * sizeof(double),
+                            cudaMemcpyHostToDevice));
+    env->params_host.assign(params_host, params_host + N * FXENV_ENV_PARAMS);
+  } else {
+    env->P.env_params_off = 0u;
+    env->params_host.clear();
+  }
+  env->P.lean = lean;
+  return invalidate_cash_bounds(env);
 }
 
 /* debug (FXENV_TIMELINE=K, timing build): copies the [K][num_envs][2] ticket start / end stamps; returns K or <0 */

@@ -55,6 +55,13 @@ struct FxBar {
   double o, h, l, c;
 };
 
+// The broker and strategy values fxenv_set_env_params can set per env, under their FxConfig names: the functions below
+// that read them are templates on the source `PC` of the values, either the FxConfig itself (one value for every env)
+// or this record (the env's row of the table).  The FxConfig instantiations are the code the library always had.
+struct FxEnvParams {
+  double commission, leverage, slippage_perc, sl_pips, tp_pips, k_sl, k_tp;
+};
+
 // Per-env scalar state while a step is being computed (registers).  Loaded from / stored to the device SoA.
 struct FxEnvRegs {
   double cash, psize, pprice, value;
@@ -107,7 +114,8 @@ FX_HD void fx_pos_update(double& psize, double& pprice, double size, double pric
 }
 
 // ---- BackBroker._execute, pseudo form (check_submitted): runs on a cash / position CLONE at created.price -------
-FX_HD void fx_pseudo_execute(const FxConfig& c, double size, double price, double& cash, double& ps, double& pp) {
+template <class PC>
+FX_HD void fx_pseudo_execute(const PC& c, double size, double price, double& cash, double& ps, double& pp) {
   double opened, closed;
   fx_pos_update(ps, pp, size, price, opened, closed);
   if (closed != 0.0) {
@@ -234,8 +242,8 @@ FX_HD void fx_rs_trade(const RS& rs, uint32_t& flags, double oldsize, double clo
 // ---- BackBroker._execute, real form.  Returns true if the order ended in Margin (=> cancel its bracket group) --
 // PLAIN (compile time): commission == 0 and leverage == 1 -- the arithmetic that those values turn into identities
 // (x / 1.0, x - 0.0) is left out; every remaining operation and its order are unchanged.
-template <bool PLAIN, class RS>
-FX_HD bool fx_execute(const FxConfig& c, FxEnvRegs& e, double size, double price, const RS& rs) {
+template <bool PLAIN, class RS, class PC>
+FX_HD bool fx_execute(const PC& c, FxEnvRegs& e, double size, double price, const RS& rs) {
   const double pprice_orig = e.pprice, oldsize = e.psize;
   double ps = e.psize, pp = e.pprice, opened, closed;
   fx_pos_update(ps, pp, size, price, opened, closed);  // pseudoupdate on a clone
@@ -371,7 +379,8 @@ FX_HD uint32_t fx_entry_begin_bar(uint32_t meta) {
 // ---- BackBroker.next, step 1: check_submitted over the entries created by the previous strategy call ------------
 // (they are the tail [k_begin, n) of the table).  Running pseudo-cash over ONE position clone, in submission order;
 // the running cash is NOT restored after a rejection (bbroker.py keeps the negative value for the rest of the batch).
-FX_HD_COLD void fx_check_submitted(const FxConfig& c, const FxEnvRegs& e, FxOrderTab& t, int k_begin) {
+template <class PC>
+FX_HD void fx_check_submitted_t(const PC& c, const FxEnvRegs& e, FxOrderTab& t, int k_begin) {
   double cash = e.cash, ps = e.psize, pp = e.pprice;
   for (int k = k_begin; k < t.n; k++) {
     const uint32_t m = t.meta[k];
@@ -395,15 +404,23 @@ FX_HD_COLD void fx_check_submitted(const FxConfig& c, const FxEnvRegs& e, FxOrde
     if (kind == FXO_PAIR) fx_kill(t, k - 1);    // a child going Margin cancels the (already accepted) group
   }
 }
+FX_HD_COLD void fx_check_submitted(const FxConfig& c, const FxEnvRegs& e, FxOrderTab& t, int k_begin) {
+  fx_check_submitted_t(c, e, t, k_begin);
+}
+FX_HD_COLD void fx_check_submitted(const FxEnvParams& c, const FxEnvRegs& e, FxOrderTab& t, int k_begin) {
+  fx_check_submitted_t(c, e, t, k_begin);
+}
 
 // Upper bound of the pseudo-cash that check_submitted can take away for one submitted entry: every pseudo-execution
 // lowers the running cash by at most |size| * price * (max(1, 1/leverage) + commission) (closing a short or opening a
 // long; the other two cases ADD cash).  A PAIR is two pseudo-executions (stop child @p0, limit child @p1).
 // If cash >= 1.001 * (sum of the bounds of all submitted entries) no order can be rejected, and the exact sequential
 // simulation can be skipped without changing any outcome (the simulation only decides accept / reject).
-FX_HD double fx_bound_per(const FxConfig& c) { return (c.leverage < 1.0 ? 1.0 / c.leverage : 1.0) + fabs(c.commission); }
+template <class PC>
+FX_HD double fx_bound_per(const PC& c) { return (c.leverage < 1.0 ? 1.0 / c.leverage : 1.0) + fabs(c.commission); }
 
-FX_HD double fx_submit_cash_bound(const FxConfig& c, uint32_t meta, double p0, double p1, double sz) {
+template <class PC>
+FX_HD double fx_submit_cash_bound(const PC& c, uint32_t meta, double p0, double p1, double sz) {
   const double per = fx_bound_per(c);
   double need = fabs(sz) * fabs(p0) * per;
   if ((meta & FXO_KIND_MASK) == FXO_PAIR) need += fabs(sz) * fabs(p1) * per;
@@ -411,13 +428,14 @@ FX_HD double fx_submit_cash_bound(const FxConfig& c, uint32_t meta, double p0, d
 }
 
 // ---- BackBroker.next, step 2: execute entry k (known to hit) in FIFO position ------------------------------------
-template <class RS>
-FX_HD void fx_exec_entry(const FxConfig& c, FxEnvRegs& e, FxOrderTab& t, int k, const FxBar& b, const RS& rs) {
+// p: the broker values (the config, or the env's row of the per-env table)
+template <class RS, class PC>
+FX_HD void fx_exec_entry(const FxConfig& c, const PC& p, FxEnvRegs& e, FxOrderTab& t, int k, const FxBar& b, const RS& rs) {
   const uint32_t m = t.meta[k];
   if (m & (FXO_DEAD | FXO_SUBMITTED)) return;
   const uint32_t kind = m & FXO_KIND_MASK;
   const bool buy = !(m & FXO_SELL);
-  const double s = c.slippage_perc;
+  const double s = p.slippage_perc;
   double px = b.o;
   bool go;
   if (kind == FXO_MARKET) { go = true; px = fx_market_price(s, buy, b); }
@@ -426,17 +444,21 @@ FX_HD void fx_exec_entry(const FxConfig& c, FxEnvRegs& e, FxOrderTab& t, int k, 
   if (!go) return;
   // Completed or Margin: either way the entry leaves the table.  A child that completes cancels its sibling, a child
   // or parent that goes Margin cancels its whole group -- for a PAIR both mean "the pair is gone".
-  const bool margin = fx_execute<false>(c, e, t.sz[k], px, rs);
+  const bool margin = fx_execute<false>(p, e, t.sz[k], px, rs);
   fx_kill(t, k);
   if (kind == FXO_PARENT) {
     if (margin) fx_kill(t, k + 1);
     else t.meta[k + 1] |= (c.children_same_bar ? FXO_ACTIVE : FXO_ACTIVATE_NEXT);
   }
 }
+template <class RS>
+FX_HD void fx_exec_entry(const FxConfig& c, FxEnvRegs& e, FxOrderTab& t, int k, const FxBar& b, const RS& rs) {
+  fx_exec_entry(c, c, e, t, k, b, rs);
+}
 
 // ---- BackBroker._get_value (shortcash valuation; the long side is un-levered) -------------------------------------
-template <bool PLAIN = false>
-FX_HD void fx_mark_to_market(const FxConfig& c, FxEnvRegs& e, double pclose) {
+template <bool PLAIN = false, class PC>
+FX_HD void fx_mark_to_market(const PC& c, FxEnvRegs& e, double pclose) {
   double unl = 0.0;
   double dvalue = e.psize * pclose;
   const double dunreal = e.psize * (pclose - e.pprice) * 1.0;
@@ -535,8 +557,11 @@ struct FxAudit {
 // ---- BTBridgeStrategy._apply_action at the current bar ------------------------------------------------------------
 // atr / atr_ready: simple-mean ATR of the env's TR deque (only read for FX_STRATEGY_ATR_SLTP).
 // au: the ATR strategy's audit record of this call (the other strategies leave it untouched).
-FX_HD void fx_apply_action(const FxConfig& c, int strategy, FxEnvRegs& e, FxOrderTab& t, int action, const FxBar& b,
-                           int pair, double atr, bool atr_ready, bool has_minutes, int64_t minutes, FxAudit& au) {
+// p: sl_pips / tp_pips / k_sl / k_tp (the config, or the env's row of the per-env table).
+template <class PC>
+FX_HD void fx_apply_action(const FxConfig& c, const PC& p, int strategy, FxEnvRegs& e, FxOrderTab& t, int action,
+                           const FxBar& b, int pair, double atr, bool atr_ready, bool has_minutes, int64_t minutes,
+                           FxAudit& au) {
   const double pos = e.psize, pclose = b.c;
   if (strategy == FX_STRATEGY_DEFAULT) {  // app/bt_bridge.py:171-190 (market orders)
     const double size = c.position_size;
@@ -554,8 +579,8 @@ FX_HD void fx_apply_action(const FxConfig& c, int strategy, FxEnvRegs& e, FxOrde
     if (action == 0) return;
     const double pip = c.pair_pip_size[pair] != 0.0 ? c.pair_pip_size[pair] : c.pip_size;
     size = c.strat_position_size;
-    sl = c.sl_pips * pip;
-    tp = c.tp_pips * pip;
+    sl = p.sl_pips * pip;
+    tp = p.tp_pips * pip;
   } else {  // direct_atr_sltp.py:110-202
     au.kind = FXENV_AU_KIND_NONE;
     size = fx_atr_size(c, e.cash, pclose);
@@ -569,8 +594,8 @@ FX_HD void fx_apply_action(const FxConfig& c, int strategy, FxEnvRegs& e, FxOrde
     if (action == 0) return;
     if (c.session_filter && !in_entry) return;
     if (!atr_ready || atr <= 0.0 || size <= 0.0 || pclose <= 0.0) return;
-    sl = c.k_sl * atr;
-    tp = c.k_tp * atr;
+    sl = p.k_sl * atr;
+    tp = p.k_tp * atr;
     if (c.use_min_frac) { const double fl = c.min_sltp_frac * pclose; if (fl > sl) sl = fl; if (fl > tp) tp = fl; }
     if (c.use_max_frac) { const double ce = c.max_sltp_frac * pclose; if (ce < sl) sl = ce; if (ce < tp) tp = ce; }
     if (tp >= pclose) tp = pclose * 0.5;
@@ -595,11 +620,20 @@ FX_HD void fx_apply_action(const FxConfig& c, int strategy, FxEnvRegs& e, FxOrde
   }
 }
 
-// The same call for callers that keep no audit.
+// The same calls with the config's values, and for callers that keep no audit.
+FX_HD void fx_apply_action(const FxConfig& c, int strategy, FxEnvRegs& e, FxOrderTab& t, int action, const FxBar& b,
+                           int pair, double atr, bool atr_ready, bool has_minutes, int64_t minutes, FxAudit& au) {
+  fx_apply_action(c, c, strategy, e, t, action, b, pair, atr, atr_ready, has_minutes, minutes, au);
+}
+template <class PC>
+FX_HD void fx_apply_action(const FxConfig& c, const PC& p, int strategy, FxEnvRegs& e, FxOrderTab& t, int action,
+                           const FxBar& b, int pair, double atr, bool atr_ready, bool has_minutes, int64_t minutes) {
+  FxAudit au;
+  fx_apply_action(c, p, strategy, e, t, action, b, pair, atr, atr_ready, has_minutes, minutes, au);
+}
 FX_HD void fx_apply_action(const FxConfig& c, int strategy, FxEnvRegs& e, FxOrderTab& t, int action, const FxBar& b,
                            int pair, double atr, bool atr_ready, bool has_minutes, int64_t minutes) {
-  FxAudit au;
-  fx_apply_action(c, strategy, e, t, action, b, pair, atr, atr_ready, has_minutes, minutes, au);
+  fx_apply_action(c, c, strategy, e, t, action, b, pair, atr, atr_ready, has_minutes, minutes);
 }
 
 // ---- app/env.py:187-204 ---------------------------------------------------------------------------------------------

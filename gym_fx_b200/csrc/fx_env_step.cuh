@@ -1,5 +1,6 @@
 // fx_env_step.cuh -- sm_90a kernels of the fused gym-fx env.step(): the step and rollout kernel templates, instantiated
-// by fx_kernels.cu (the variants without truncation) and fx_kernels_trunc.cu (those with it) through fx_variant_lookup.
+// through fx_variant_lookup by fx_kernels.cu, fx_kernels_trunc.cu, fx_kernels_params.cu and fx_kernels_params_trunc.cu
+// (the variants without / with truncation and per-env parameters, see fx_kernels.cuh).
 //
 // fx_step_env<STRATEGY, REWARD, V> is the whole env-step of ONE env by ONE warp (no block barrier anywhere):
 //
@@ -771,6 +772,28 @@ struct FxStamps {
 #endif
 };
 
+// The broker and strategy values of an env-step (FxEnvParams, fx_core.cuh): in the kernels without FX_V_PARAMS the
+// configuration itself (a reference to the kernel parameters, as before), in those with it the env's row of the table,
+// loaded one field per lane (`v`, lanes 0..6) with the state and broadcast here.
+template <bool PARAMS>
+struct FxStepParams {
+  static __device__ __forceinline__ const FxConfig& get(const FxConfig& c, double) { return c; }
+};
+template <>
+struct FxStepParams<true> {
+  static __device__ __forceinline__ FxEnvParams get(const FxConfig&, double v) {
+    FxEnvParams p;
+    p.commission = __shfl_sync(FX_FULL, v, FXENV_PARAM_COMMISSION);
+    p.leverage = __shfl_sync(FX_FULL, v, FXENV_PARAM_LEVERAGE);
+    p.slippage_perc = __shfl_sync(FX_FULL, v, FXENV_PARAM_SLIPPAGE);
+    p.sl_pips = __shfl_sync(FX_FULL, v, FXENV_PARAM_SL_PIPS);
+    p.tp_pips = __shfl_sync(FX_FULL, v, FXENV_PARAM_TP_PIPS);
+    p.k_sl = __shfl_sync(FX_FULL, v, FXENV_PARAM_K_SL);
+    p.k_tp = __shfl_sync(FX_FULL, v, FXENV_PARAM_K_TP);
+    return p;
+  }
+};
+
 // One env-step of one env by one warp (everything between the cross-kernel dependency wait and the release).
 // V: the variant key (FX_V_*).
 // CARRY (fx_rollout_kernel): the step leaves the env's scalar state in ws.carry and returns true if that record is valid;
@@ -791,6 +814,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   const FxStepOut o{obs, obs16, reward, reward64, terminated, step_row, obs_slot_row, stride16};
   constexpr bool FAST5 = (V & FX_V_FAST5) != 0, LEAN = (V & FX_V_LEAN) != 0, RESIDENT = (V & FX_V_RESIDENT) != 0;
   constexpr bool AUDIT = (V & FX_V_AUDIT) != 0, REPEAT = (V & FX_V_REPEAT) != 0, TRUNC = (V & FX_V_TRUNC) != 0;
+  constexpr bool PARAMS = (V & FX_V_PARAMS) != 0;
   constexpr bool ATR = STRATEGY == FX_STRATEGY_ATR_SLTP;
   static_assert(!REPEAT || CARRY, "substeps hand the env over through the carry record");
   static_assert(!RESIDENT || CARRY, "the shared copy of the order table lives as long as the carry record");
@@ -813,6 +837,8 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   double2 nb_oh, nb_lc;
   double nb_price, rsv = 0.0;
   int32_t dec = 0;  // TRUNC: decisions of the episode before this step
+  double prow = 0.0;  // PARAMS: field `lane` of the env's row (lanes 0..6)
+  if (PARAMS && lane < FXENV_ENV_PARAMS) prow = fx_env_params(P)[(int64_t)env * FXENV_ENV_PARAMS + lane];
   if (CARRY && carry_in) {  // the record this warp left behind one step ago (shared memory: broadcast reads)
     const double* __restrict__ cr = ws.carry;
     const int2 ft = *reinterpret_cast<const int2*>(cr + FX_CARRY_FLAGS_T);
@@ -907,6 +933,9 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
     return false;  // (the carry record does not follow resets / ended episodes: the next step reloads the arrays)
   }
 
+  // the values the broker and the strategy read (the configuration's, or the env's row: PARAMS)
+  const auto& pc = FxStepParams<PARAMS>::get(c, prow);
+
   // ---- step <-> bar timeline (SURVEY A.1): the first step does not advance; later steps advance or exhaust
   bool exhausted = false, advance = false;
   if (!(flags & FX_FLAG_STARTED)) flags |= FX_FLAG_STARTED;
@@ -964,7 +993,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
           FxOrderTab tg;
           tg.meta = gmeta; tg.p0 = gp0; tg.p1 = gp1; tg.sz = gsz;
           tg.n = n; tg.cap = P.cap; tg.dirty_from = n; tg.ndead = 0; tg.sub_need = 0.0; tg.bound_per = 0.0;
-          fx_check_submitted(c, e, tg, first_sub);  // clears SUBMITTED / marks DEAD in place
+          fx_check_submitted(pc, e, tg, first_sub);  // clears SUBMITTED / marks DEAD in place
           __syncwarp();
           first_sub = n;    // nothing left to accept in the pass below
           reload0 = true;   // the prefetched chunk may be stale
@@ -994,7 +1023,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
           }
           carry = 0u;
           double px_lane = 0.0;  // execution price of this lane's entry, should it trade on this bar
-          const bool hit = fx_entry_fill(LEAN ? 0.0 : c.slippage_perc, m, p0, p1, b, px_lane);
+          const bool hit = fx_entry_fill(LEAN ? 0.0 : pc.slippage_perc, m, p0, p1, b, px_lane);
           uint32_t hm = __ballot_sync(FX_FULL, valid && !(m & FXO_DEAD) && hit);
           while (hm) {
             const int l = __ffs(hm) - 1;
@@ -1004,7 +1033,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
             const uint32_t kind = bm & FXO_KIND_MASK;
             if (kind == FXO_PAIR && !(bm & FXO_ACTIVE)) continue;
             // Completed or Margin: either way the entry leaves the table (a PAIR: sibling / group cancelled)
-            const bool margin = fx_execute<LEAN>(c, e, __shfl_sync(FX_FULL, sz, l), __shfl_sync(FX_FULL, px_lane, l), rs);
+            const bool margin = fx_execute<LEAN>(pc, e, __shfl_sync(FX_FULL, sz, l), __shfl_sync(FX_FULL, px_lane, l), rs);
             any_fill = true;
             n_fills++;
             if (lane == l) m |= FXO_DEAD;
@@ -1026,7 +1055,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
         n_live = w;
         ts.put(lane, 4, ((long long)n << 32) | (long long)n_fills);  // debug: table size, fills
       }
-      fx_mark_to_market<LEAN>(c, e, b.c);
+      fx_mark_to_market<LEAN>(pc, e, b.c);
       // DrawDown analyzer: one notify_fund + next per bar.  With no position and no execution the value is the one of
       // the previous bar and nothing can change.
       if (any_fill || e.psize != 0.0) {
@@ -1092,10 +1121,10 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       // bound is accumulated by fx_push and kept in the env state for the next step
       FxOrderTab tg;
       tg.meta = gmeta; tg.p0 = gp0; tg.p1 = gp1; tg.sz = gsz;
-      tg.n = n_live; tg.cap = P.cap; tg.dirty_from = n_live; tg.ndead = 0; tg.sub_need = 0.0; tg.bound_per = LEAN ? 1.0 : fx_bound_per(c);
+      tg.n = n_live; tg.cap = P.cap; tg.dirty_from = n_live; tg.ndead = 0; tg.sub_need = 0.0; tg.bound_per = LEAN ? 1.0 : fx_bound_per(pc);
       FxAudit au;
       au.kind = FXENV_AU_KIND_NONE;
-      fx_apply_action(c, STRATEGY, e, tg, action, b, pair, atr, atr_ready, has_min, minutes, au);
+      fx_apply_action(c, pc, STRATEGY, e, tg, action, b, pair, atr, atr_ready, has_min, minutes, au);
       if (AUDIT && au.kind != FXENV_AU_KIND_NONE) fx_audit_store(P, env, lane, au, start + t, b.c);
       n_final = tg.n;
       sub_need_new = tg.sub_need;
@@ -1430,29 +1459,30 @@ fx_rollout_kernel(const __grid_constant__ FxKernelParams P, const char* __restri
   }
 }
 
-// The kernels of one (strategy, reward, key) of the half TRUNC (0 or FX_V_TRUNC): none for a key of the other half or one
-// that fx_variant_valid rejects.  The step kernel has no resident order table, so keys with and without FX_V_RESIDENT
-// share it.
-template <unsigned TRUNC, int STRATEGY, int REWARD, unsigned V>
+// The kernels of one (strategy, reward, key) of the half HALF (its FX_V_TRUNC | FX_V_PARAMS bits): none for a key of
+// another half or one that fx_variant_valid rejects.  The step kernel has no resident order table, so keys with and
+// without FX_V_RESIDENT share it.
+constexpr unsigned FX_V_HALF = FX_V_TRUNC | FX_V_PARAMS;
+template <unsigned HALF, int STRATEGY, int REWARD, unsigned V>
 FxEnvKernels fx_variant_entry() {
-  if constexpr ((V & FX_V_TRUNC) == TRUNC && fx_variant_valid(STRATEGY, V))
+  if constexpr ((V & FX_V_HALF) == HALF && fx_variant_valid(STRATEGY, V))
     return {fx_step_kernel<STRATEGY, REWARD, V & ~FX_V_RESIDENT>, fx_rollout_kernel<STRATEGY, REWARD, V>};
   else
     return {nullptr, nullptr};
 }
 
-template <unsigned TRUNC, size_t... I>
+template <unsigned HALF, size_t... I>
 FxEnvKernels fx_variant_table(int strategy, int reward, unsigned key, std::index_sequence<I...>) {
   static const FxEnvKernels table[] = {
-      fx_variant_entry<TRUNC, (int)(I / (FX_N_REWARDS * FX_V_KEYS)), (int)(I / FX_V_KEYS % FX_N_REWARDS), (unsigned)(I % FX_V_KEYS)>()...};
+      fx_variant_entry<HALF, (int)(I / (FX_N_REWARDS * FX_V_KEYS)), (int)(I / FX_V_KEYS % FX_N_REWARDS), (unsigned)(I % FX_V_KEYS)>()...};
   return table[((size_t)strategy * FX_N_REWARDS + (size_t)reward) * FX_V_KEYS + key];
 }
 
-// The lookup over every (strategy, reward, key) whose FX_V_TRUNC bit is TRUNC: the translation unit that calls it
-// instantiates exactly those kernels.
-template <unsigned TRUNC>
+// The lookup over every (strategy, reward, key) whose FX_V_TRUNC | FX_V_PARAMS bits are HALF: the translation unit that
+// calls it instantiates exactly those kernels.
+template <unsigned HALF>
 FxEnvKernels fx_variant_lookup(int strategy, int reward, unsigned key) {
-  return fx_variant_table<TRUNC>(strategy, reward, key, std::make_index_sequence<FX_N_STRATEGIES * FX_N_REWARDS * FX_V_KEYS>());
+  return fx_variant_table<HALF>(strategy, reward, key, std::make_index_sequence<FX_N_STRATEGIES * FX_N_REWARDS * FX_V_KEYS>());
 }
 
 }  // namespace

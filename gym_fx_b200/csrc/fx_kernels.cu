@@ -1,6 +1,7 @@
 // fx_kernels.cu -- sm_90a kernels of the fused gym-fx env.step(): the host side (configuration, kernel choice,
 // launches), the reset / observe / statistics kernels, and the step / rollout kernels of fx_env_step.cuh without
-// truncation (those with it: fx_kernels_trunc.cu).
+// truncation and per-env parameters (the other halves: fx_kernels_trunc.cu, fx_kernels_params.cu,
+// fx_kernels_params_trunc.cu).
 #include <cstdlib>
 
 #include "fx_env_step.cuh"
@@ -106,13 +107,18 @@ unsigned fx_variant_key(const FxKernelParams& P) {
   if (P.audit != nullptr && P.cfg.strategy == FX_STRATEGY_ATR_SLTP) key |= FX_V_AUDIT;
   if (P.repeat > 1) key |= FX_V_REPEAT;
   if (fx_trunc_on(P)) key |= FX_V_TRUNC;
+  if (P.env_params_off != 0u) key |= FX_V_PARAMS;
   return key;
 }
 
-// the kernels of a key: from this translation unit's half of the table, or from fx_kernels_trunc.cu's
+// the kernels of a key: from this translation unit's part of the table, or from the unit that holds the key's half
 FxEnvKernels env_kernels(const FxKernelParams& P, unsigned key) {
-  if (key & FX_V_TRUNC) return fx_trunc_kernels(P.cfg.strategy, P.cfg.reward, key);
-  return fx_variant_lookup<0u>(P.cfg.strategy, P.cfg.reward, key);
+  switch (key & (FX_V_TRUNC | FX_V_PARAMS)) {
+    case FX_V_TRUNC: return fx_trunc_kernels(P.cfg.strategy, P.cfg.reward, key);
+    case FX_V_PARAMS: return fx_params_kernels(P.cfg.strategy, P.cfg.reward, key);
+    case FX_V_PARAMS | FX_V_TRUNC: return fx_params_trunc_kernels(P.cfg.strategy, P.cfg.reward, key);
+    default: return fx_variant_lookup<0u>(P.cfg.strategy, P.cfg.reward, key);
+  }
 }
 
 }  // namespace
@@ -127,9 +133,10 @@ int fx_order_smem_choice(const FxKernelParams& P, int force) {
   return (cta <= 227 * 1024 && ctas * (cta + 1024) <= 228 * 1024) ? 1 : 0;
 }
 
-// Attributes of one half of the step / rollout instantiations (trunc: 0 or FX_V_TRUNC) and the persistent grid: dynamic
-// shared memory above the 48 KB default needs an explicit opt-in per kernel.  P.order_smem is decided.
-static cudaError_t fx_configure_variants(FxKernelParams& P, unsigned trunc) {
+// Attributes of one half of the step / rollout instantiations (half: its FX_V_TRUNC | FX_V_PARAMS bits) and the
+// persistent grid: dynamic shared memory above the 48 KB default needs an explicit opt-in per kernel.  P.order_smem is
+// decided.
+static cudaError_t fx_configure_variants(FxKernelParams& P, unsigned half) {
   const size_t smem = step_smem_bytes(P), rsmem = rollout_smem_bytes(P, P.order_smem != 0);
   // ask for enough shared-memory carve-out that FX_MIN_BLOCKS CTAs (+1 KB system use each) fit on an SM
   const int pct = carveout_pct(FX_MIN_BLOCKS, smem);
@@ -138,8 +145,8 @@ static cudaError_t fx_configure_variants(FxKernelParams& P, unsigned trunc) {
   const int sms = P.num_sms;
   // every key of the handle's fast path and order-table choice: LEAN or not (which one runs is only known once the
   // candle tables are loaded), both states of the bracket audit (ATR strategy) and both states of the action repeat
-  const unsigned fixed = FX_V_FAST5 | FX_V_RESIDENT | FX_V_TRUNC;
-  const unsigned want = (fx_variant_key(P) & (FX_V_FAST5 | FX_V_RESIDENT)) | trunc;
+  const unsigned fixed = FX_V_FAST5 | FX_V_RESIDENT | FX_V_TRUNC | FX_V_PARAMS;
+  const unsigned want = (fx_variant_key(P) & (FX_V_FAST5 | FX_V_RESIDENT)) | half;
   for (unsigned key = 0u; key < FX_V_KEYS; key++) {
     if ((key & fixed) != want || !fx_variant_valid(P.cfg.strategy, key)) continue;
     const FxEnvKernels k = env_kernels(P, key);
@@ -188,12 +195,26 @@ cudaError_t fx_configure_kernels(FxKernelParams& P) {
 
 cudaError_t fx_configure_trunc_kernels(FxKernelParams& P) { return fx_configure_variants(P, FX_V_TRUNC); }
 
+cudaError_t fx_configure_params_kernels(FxKernelParams& P, unsigned trunc) {
+  return fx_configure_variants(P, FX_V_PARAMS | (trunc & FX_V_TRUNC));
+}
+
 // The LEAN contract of the specialised kernels (see fx_uses_running_stats): everything here is a property of the
-// resolved configuration except `tame_data`, which is known once every pair's candle table has been loaded.
-bool fx_config_is_lean(const FxKernelParams& P) {
+// resolved configuration except `tame_data`, which is known once every pair's candle table has been loaded.  With a
+// per-env table (rows_host) its rows' costs decide instead of the configuration's: the LEAN kernels leave commission,
+// leverage and slippage out, and take only sl / tp / k_sl / k_tp from the row.
+bool fx_config_is_lean(const FxKernelParams& P, const double* rows_host) {
   const FxConfig& c = P.cfg;
   if (P.fast_features != 5 || P.debug != 0 || !P.tame_data || P.any_binary) return false;
-  if (c.action_mode != FX_ACTION_DISCRETE || c.commission != 0.0 || c.leverage != 1.0 || c.slippage_perc != 0.0) return false;
+  if (c.action_mode != FX_ACTION_DISCRETE) return false;
+  if (rows_host) {
+    for (int i = 0; i < c.num_envs; i++) {
+      const double* r = rows_host + (size_t)i * FXENV_ENV_PARAMS;
+      if (r[FXENV_PARAM_COMMISSION] != 0.0 || r[FXENV_PARAM_LEVERAGE] != 1.0 || r[FXENV_PARAM_SLIPPAGE] != 0.0) return false;
+    }
+  } else if (c.commission != 0.0 || c.leverage != 1.0 || c.slippage_perc != 0.0) {
+    return false;
+  }
   if (c.children_same_bar || c.preproc != FX_PREPROC_FEATURE_WINDOW || c.scaling != FX_SCALING_ROLLING) return false;
   if (!(c.feature_clip > 0.0) || !c.include_price_window || !c.include_agent_state || (c.window_size & 3) || c.price_col > 4) return false;
   return true;

@@ -91,12 +91,24 @@ struct FxKernelParams {
   // of the handle like the repeat; while either is set the host launches the truncation instantiations (fx_trunc_on).
   int32_t max_steps;
   uint32_t trunc_flags;
+  // per-env broker and strategy values (fxenv_set_env_params): byte offset of the [N][FXENV_ENV_PARAMS] FxEnvParams rows
+  // in the allocation of `seq` (fx_env_params), or 0 (off: the FxConfig values; the kernels without FX_V_PARAMS run).  A
+  // setting of the handle outside the slab, like the audit.  An offset in the 4 bytes of padding before ep_steps rather
+  // than a pointer of its own: a new 8-byte field would grow the kernel parameters and move every kernel argument after
+  // them, changing the code of every existing kernel.  The table stays put while it is on, so that cached graphs read
+  // values updated in place.
+  uint32_t env_params_off;
   // [N] decisions of the current episode (a column of the state slab, so snapshots carry it; zeroed by fx_reset_env).
   // Addressed from here rather than from FxDeviceState so that no existing kernel parameter moves.
   int32_t* ep_steps;
 };
 
 __host__ __device__ inline bool fx_trunc_on(const FxKernelParams& P) { return P.max_steps > 0 || P.trunc_flags != 0u; }
+
+// the per-env parameter table while it is on (env_params_off != 0)
+__host__ __device__ inline const double* fx_env_params(const FxKernelParams& P) {
+  return reinterpret_cast<const double*>(reinterpret_cast<const char*>(P.seq) + P.env_params_off);
+}
 
 // warps (= envs) per CTA of the step kernel.  One warp per CTA lets the second wave back-fill SM slots as soon as a
 // single env finishes.
@@ -147,7 +159,11 @@ cudaError_t fx_configure_kernels(FxKernelParams& P);
 // the same for the truncation instantiations; deferred to the first fxenv_set_time_limit that turns truncation on, so
 // that a handle without a time limit never loads their module
 cudaError_t fx_configure_trunc_kernels(FxKernelParams& P);
-bool fx_config_is_lean(const FxKernelParams& P);
+// the same for the per-env parameter instantiations (FX_V_PARAMS), with (trunc = FX_V_TRUNC) or without truncation;
+// deferred to the first fxenv_set_env_params
+cudaError_t fx_configure_params_kernels(FxKernelParams& P, unsigned trunc);
+// rows_host: the per-env table ([N][FXENV_ENV_PARAMS]) whose costs decide instead of the config's, or nullptr
+bool fx_config_is_lean(const FxKernelParams& P, const double* rows_host = nullptr);
 cudaError_t fx_launch_rollout(const FxKernelParams& P, const void* actions, float* obs, int obs_slots, float* reward,
                               uint8_t* terminated, const FxChunkPlan& plan, unsigned seq_base, unsigned ticket_base,
                               bool reset_words, cudaStream_t stream);
@@ -164,7 +180,8 @@ enum : unsigned {
   FX_V_AUDIT = 8u,     // the bracket audit store (fxenv_set_bracket_audit)
   FX_V_REPEAT = 16u,   // the action repeat (fxenv_set_action_repeat, repeat > 1)
   FX_V_TRUNC = 32u,    // decision counts and truncation (fxenv_set_time_limit, fx_trunc_on)
-  FX_V_KEYS = 64u
+  FX_V_PARAMS = 64u,   // per-env broker and strategy values (fxenv_set_env_params, env_params_off)
+  FX_V_KEYS = 128u
 };
 enum { FX_N_STRATEGIES = FX_STRATEGY_ATR_SLTP + 1, FX_N_REWARDS = FX_REWARD_DD + 1 };
 // The keys that have kernels: LEAN needs the fast path and the audit the ATR strategy.  (FX_V_RESIDENT selects a rollout
@@ -182,6 +199,10 @@ struct FxEnvKernels {
   FxStepKernelFn step;
   FxRolloutKernelFn rollout;
 };
-// the kernels of a key with FX_V_TRUNC (fx_kernels_trunc.cu; fx_kernels.cu holds those without it)
+// The kernels are split over four translation units by the two bits FX_V_TRUNC and FX_V_PARAMS (the "half" of a key):
+// fx_kernels.cu holds the keys with neither, fx_kernels_trunc.cu those with FX_V_TRUNC only, fx_kernels_params.cu those
+// with FX_V_PARAMS only and fx_kernels_params_trunc.cu those with both.
 FxEnvKernels fx_trunc_kernels(int strategy, int reward, unsigned key);
+FxEnvKernels fx_params_kernels(int strategy, int reward, unsigned key);
+FxEnvKernels fx_params_trunc_kernels(int strategy, int reward, unsigned key);
 FxChunkPlan fx_rollout_plan(const FxKernelParams& P, int n_steps);  // the host's ticket accounting needs n_rounds

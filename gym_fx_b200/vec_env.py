@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _native
-from .config import FxConfig, obs_dim, obs_layout
+from .config import FxConfig, env_params_table, obs_dim, obs_layout
 
 
 class VecFxEnv:
@@ -67,6 +67,7 @@ class VecFxEnv:
         self._audit = None  # (ring [N, capacity, 8], written [N], read cursor [N]) while the bracket audit is on
         self.action_repeat = (1, False)  # (k, hold): set_action_repeat
         self.time_limit = (0, False)  # (max_steps, truncate_window): set_time_limit
+        self.env_params: Optional[np.ndarray] = None  # float64 [N, 7] host copy of the per-env table (set_env_params)
 
     # ------------------------------------------------------------------ lifecycle
     def close(self):
@@ -470,6 +471,27 @@ class VecFxEnv:
         else:   # off: back to the zero-overhead views of the 0 / 1 buffer
             self._term_bool = None
             self.truncated.zero_()
+
+    # ------------------------------------------------------------------ per-env broker / strategy parameters
+    def set_env_params(self, commission=None, leverage=None, slippage=None, sl_pips=None, tp_pips=None, k_sl=None,
+                       k_tp=None):
+        """Give each env its own broker costs and bracket settings (include/fxenv.h fxenv_set_env_params): commission,
+        leverage and slippage of the broker, sl_pips / tp_pips of direct_fixed_sltp, k_sl / k_tp of direct_atr_sltp.  Each
+        argument is a scalar (every env) or an [N] array / tensor; a field left as None keeps the config's value.  With
+        every field None (set_env_params(None)) the table is turned off and every env uses the config again.  Fields
+        the strategy does not use are ignored.  A setting of the handle: snapshots and reset() keep it.  New values apply
+        from the next step on; updating the values while the table stays on keeps the cached step_many / rollout graphs.
+        Synchronous.  Bad values (not finite, leverage <= 0, slippage outside [0, 1), a wrong length) raise ValueError
+        and leave the table in force as it was.  The host copy of the table in force is `env_params` (None when off)."""
+        fields = dict(commission=commission, leverage=leverage, slippage=slippage, sl_pips=sl_pips, tp_pips=tp_pips,
+                      k_sl=k_sl, k_tp=k_tp)
+        table = None if all(v is None for v in fields.values()) else env_params_table(self.cfg, **fields)
+        with torch.cuda.device(self.device):
+            rc = self.L.fxenv_set_env_params(self._h, None if table is None else table.ctypes.data)
+        if rc == -1:
+            raise ValueError(self.L.fxenv_last_error(self._h).decode())
+        _native.check(self.L, self._h, rc, "fxenv_set_env_params")
+        self.env_params = table
 
     # ------------------------------------------------------------------ closed loop (policy on the device)
     def make_policy(self, weights=None, hidden: Optional[int] = None) -> "FusedPolicy":

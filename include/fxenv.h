@@ -22,6 +22,7 @@
  *                                  continuous actions are the Box(-1, 1, (1,)) of app/env.py:71-80, 187-204
  *   fxenv_set_action_repeat        (no counterpart: k bars per step, one decision per step; its contract below)
  *   fxenv_set_time_limit           (no counterpart: Gymnasium's max_episode_steps and truncation; its contract below)
+ *   fxenv_set_env_params           (no counterpart: per-env commission / leverage / slippage / SL / TP; its contract below)
  *
  * Conventions: every function returns 0 on success, <0 on error (see FXENV_E_*); fxenv_last_error() gives the
  * message.  No exceptions or aborts cross the ABI.  The library owns env state (device struct-of-arrays) behind
@@ -381,6 +382,32 @@ int fxenv_set_action_repeat(FxEnv* env, int32_t repeat, uint32_t flags);
 #define FXENV_DONE_TERMINATED 1
 #define FXENV_DONE_TRUNCATED 2
 int fxenv_set_time_limit(FxEnv* env, int32_t max_steps, uint32_t flags);
+
+/* ---- per-env broker and strategy parameters (no reference counterpart: one reference env has one configuration; a
+ * handle of N envs can run N of them, e.g. a backtest grid over SL x TP x commission, or costs drawn per env for RL) ----
+ * params_host: float64 [num_envs][FXENV_ENV_PARAMS] row-major, or NULL (off: every env uses the FxConfig values).
+ * Row i replaces, for env i only, the FxConfig field of the same meaning everywhere the library uses it:
+ *   FXENV_PARAM_COMMISSION / _LEVERAGE / _SLIPPAGE   commission, leverage, slippage_perc of the broker: executions,
+ *       check_submitted's pseudo-executions and its cash bound, the mark to market, every slipped fill price, margin;
+ *   FXENV_PARAM_SL_PIPS / _TP_PIPS                   sl_pips, tp_pips of direct_fixed_sltp;
+ *   FXENV_PARAM_K_SL / _K_TP                         k_sl, k_tp of direct_atr_sltp.
+ * Fields the strategy does not use are accepted and ignored.  Not replaced: strat_leverage (ATR rel-volume sizing),
+ * position sizes, pip sizes, initial cash, every preprocessor and reward field.
+ * Validation, per row, as fxenv_create checks the config: every field finite, leverage > 0, 0 <= slippage < 1.  A bad
+ * row is FXENV_E_INVALID (fxenv_last_error names the env and the field) and leaves the table in force before the call.
+ * The table belongs to the handle, like the time limit: fxenv_state_bytes, snapshots, fxenv_reset and fxenv_set_state
+ * neither include nor change it.  Synchronous: the call waits for the device before it copies.
+ *   A call that keeps the table on and the kernel choice (fxenv_debug_lean) the same updates the values in place: the
+ *     cached step-many graphs and the policies' rollout graphs stay valid and read the new values.  Turning the table
+ *     on or off, or a change of the LEAN choice, drops those graphs as the other setters do.
+ *   LEAN (fxenv_debug_lean): decided on the table's values while it is on -- every row with commission 0, leverage 1 and
+ *     slippage 0, and the rest of the configuration qualifying.
+ *   New values apply from the next env-step on.  Orders already in the table keep their stop / limit prices; their
+ *     later fills, the cash bound of orders submitted before the call included, use the new costs. */
+#define FXENV_ENV_PARAMS 7
+enum { FXENV_PARAM_COMMISSION = 0, FXENV_PARAM_LEVERAGE, FXENV_PARAM_SLIPPAGE,
+       FXENV_PARAM_SL_PIPS, FXENV_PARAM_TP_PIPS, FXENV_PARAM_K_SL, FXENV_PARAM_K_TP };
+int fxenv_set_env_params(FxEnv* env, const double* params_host);
 
 /* ---- closed loop: a policy on the device between the steps ------------------------------------------------------
  * Replaces the caller loop of app/main.py:57-65 (`action = strategy.decide_action(obs, info, step); env.step(action)`)
