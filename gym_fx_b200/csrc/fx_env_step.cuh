@@ -4,8 +4,8 @@
 //
 // fx_step_env<STRATEGY, REWARD, V> is the whole env-step of ONE env by ONE warp (no block barrier anywhere):
 //
-//   load     one round trip: the env's state scalars, its action, the candle of this step (saved by the previous step)
-//            and the first 32 orders of its table;
+//   load     one round trip: the env's state scalars (fx_step_load), its action, the candle of this step (saved by the
+//            previous step) and the first 32 orders of its table;
 //   prefetch lane 0 issues TMA bulk copies (cp.async.bulk + mbarrier) of the env's candle window (W rows x n_cols fp64,
 //            one contiguous span of the table) and of the bar's z-score statistics into the warp's shared memory;
 //            they land while the broker runs;
@@ -14,7 +14,8 @@
 //            per lane (ballot), the few orders that trade are executed in FIFO order by uniform scalar fp64 code
 //            (fx_core.cuh) with their fields broadcast by shuffle, then stable compaction + write-back of what
 //            changed.  check_submitted is decided by a rigorous cash bound (the exact sequential simulation is a cold
-//            path).  Then apply_action, publish, reward, write-back;
+//            path).  Then the drawdown analyzer (fx_step_drawdown), apply_action, publish, reward (fx_step_reward),
+//            write-back;
 //   observe  the observation row ([W,F] z-scored features | prices | returns | 4 agent scalars) is produced from the
 //            staged window: fp64 math, coalesced fp32 streaming stores (>99% of the bytes).
 //
@@ -794,6 +795,134 @@ struct FxStepParams<true> {
   }
 };
 
+// ---- phases of fx_step_env as functions of their own: the state load, the drawdown analyzer and the reward ---------
+// Each takes what it reads by value or const reference, returns what it produces, and takes by reference only what it
+// updates (the env's FxEnvRegs, the lane's run-statistics field).  They are inlined and compile to the same code as
+// when written out.  The other phases stay written out in fx_step_env: cut into functions they compile differently.
+
+// The env's scalar state besides FxEnvRegs, as fx_step_load reads it (the state arrays or the carry record)
+struct FxStepState {
+  uint32_t flags;
+  int32_t t, total_bars;
+  int64_t start;
+  int n, n_acc;     // entries of the order table; the first one created by the previous strategy call
+  double sub_need;  // check_submitted cash bound of the entries [n_acc, n)
+  int32_t dec;      // TRUNC: decisions of the episode before this step
+  FxBar nb;         // the candle this step works on, saved by the previous step (FxDeviceState::nbar)
+  double nb_price;  // its price column
+};
+
+// ---- round trip 1: one batch of independent state loads (invariants: see FxDeviceState); rsv: field `lane` of the
+//      DrawDown / TradeAnalyzer / SQN record
+template <bool TRUNC, bool CARRY>
+__device__ __forceinline__ FxStepState fx_step_load(const FxKernelParams& P, const int env, const int lane, const WarpSmem& ws,
+                                                    const bool carry_in, FxEnvRegs& e, double& rsv) {
+  const FxDeviceState& st = P.st;
+  FxStepState s;
+  s.dec = 0;
+  if (CARRY && carry_in) {  // the record this warp left behind one step ago (shared memory: broadcast reads)
+    const double* __restrict__ cr = ws.carry;
+    const int2 ft = *reinterpret_cast<const int2*>(cr + FX_CARRY_FLAGS_T);
+    const int2 bn = *reinterpret_cast<const int2*>(cr + FX_CARRY_BARS_N);
+    const int2 at = *reinterpret_cast<const int2*>(cr + FX_CARRY_NACC_TRADES);
+    s.flags = (uint32_t)ft.x; s.t = ft.y; s.total_bars = bn.x; s.n = bn.y; s.n_acc = at.x; e.trades = at.y;
+    s.start = *reinterpret_cast<const long long*>(cr + FX_CARRY_START);
+    s.sub_need = cr[FX_CARRY_SUBNEED];
+    e.cash = cr[FX_CARRY_CASH]; e.psize = cr[FX_CARRY_PSIZE]; e.pprice = cr[FX_CARRY_PPRICE]; e.equity = cr[FX_CARRY_EQUITY];
+    e.commission_paid = cr[FX_CARRY_COMM];
+    s.nb.o = cr[FX_CARRY_NBAR]; s.nb.h = cr[FX_CARRY_NBAR + 1]; s.nb.l = cr[FX_CARRY_NBAR + 2]; s.nb.c = cr[FX_CARRY_NBAR + 3];
+    s.nb_price = cr[FX_CARRY_NBAR + 4];
+    if (TRUNC) s.dec = *fx_carry_dec(ws);
+    if (lane < FX_RS_N) rsv = cr[FX_CARRY_RSTATS + lane];
+  } else {
+    s.flags = st.flags[env];
+    s.t = st.t[env];
+    s.total_bars = st.total_bars[env];
+    s.start = st.start[env];
+    s.n = st.n_orders[env];
+    s.n_acc = st.n_acc[env];
+    s.sub_need = st.sub_need[env];
+    e.cash = st.cash[env]; e.psize = st.psize[env]; e.pprice = st.pprice[env]; e.equity = st.equity[env];
+    e.commission_paid = st.commission_paid[env]; e.trades = st.trades[env];
+    // the candle this call works on was saved by the previous call (FxDeviceState::nbar): it travels in this same round trip
+    const double2* __restrict__ nb2 = reinterpret_cast<const double2*>(st.nbar + (int64_t)env * 6);
+    const double2 nb_oh = nb2[0], nb_lc = nb2[1];
+    s.nb.o = nb_oh.x; s.nb.h = nb_oh.y; s.nb.l = nb_lc.x; s.nb.c = nb_lc.y;
+    s.nb_price = st.nbar[(int64_t)env * 6 + 4];
+    if (TRUNC) s.dec = P.ep_steps[env];
+    if (lane < FX_RS_N) rsv = st.rstats[(int64_t)env * FX_RS_N + lane];  // DrawDown / TradeAnalyzer / SQN state
+  }
+  e.value = e.equity;
+  return s;
+}
+
+// DrawDown analyzer: one notify_fund + next per bar.  With no position and no execution the value is the one of
+// the previous bar and nothing can change.
+__device__ __forceinline__ void fx_step_drawdown(const FxDeviceState& st, const int env, const int lane, const FxEnvRegs& e,
+                                                 const bool any_fill, double& rsv) {
+  if (any_fill || e.psize != 0.0) {
+    // fx_rs_drawdown in the lane layout: ONE broadcast (the peak), then lanes 0 / 1 / 2 each test their own field;
+    // the percent needs its division only when it can set a new maximum.  The record goes back to memory only when
+    // something in it changed (an execution, a new peak, a new maximum drawdown).
+    const double peak0 = __shfl_sync(FX_FULL, rsv, FX_RS_DD_MAXVALUE);
+    const double peak = e.value > peak0 ? e.value : peak0;
+    const double md = peak - e.value;
+    double cand = (lane == FX_RS_DD_MAXVALUE) ? peak : md;
+    const bool pct_may = (lane == FX_RS_DD_MAX_PCT) && (100.0 * md > rsv * peak * 0.999999);
+    if (__any_sync(FX_FULL, pct_may)) { if (lane == FX_RS_DD_MAX_PCT) cand = pct_may ? 100.0 * md / peak : 0.0; }
+    else if (lane == FX_RS_DD_MAX_PCT) cand = 0.0;
+    const bool up = (lane <= FX_RS_DD_MAX_PCT) && (cand > rsv);
+    if (up) rsv = cand;
+    if (any_fill || __any_sync(FX_FULL, up)) { if (lane < FX_RS_N) st.rstats[(int64_t)env * FX_RS_N + lane] = rsv; }
+  }
+}
+
+// ---- reward plugin (app/env.py:148-155)
+template <int REWARD, bool CARRY>
+__device__ __forceinline__ double fx_step_reward(const FxKernelParams& P, const FxEnvRegs& e, const int env, const int lane,
+                                                 const WarpSmem& ws, const bool carry_in) {
+  const FxConfig& c = P.cfg;
+  const FxDeviceState& st = P.st;
+  double r;
+  if (REWARD == FX_REWARD_PNL) {
+    r = fx_reward_pnl(c, e);
+  } else if (REWARD == FX_REWARD_DD) {
+    double peak = st.dd_peak[env];
+    int32_t last = st.dd_last_step[env];
+    r = fx_reward_dd(c, e, peak, last);
+    if (lane == 0) { st.dd_peak[env] = peak; st.dd_last_step[env] = last; }
+  } else {
+    // deque of per-step returns: stage the ring in shared memory (coalesced), push, evaluate in Python order
+    const int Wn = c.sharpe_window;
+    double* gring = st.sh_ring + (int64_t)env * Wn;
+    int32_t len, head, last;
+    if (CARRY && carry_in) {  // this warp ran the env's previous step: its copy of the deque is current
+      const int2 lh = *reinterpret_cast<const int2*>(ws.carry + FX_CARRY_SHARPE);
+      len = lh.x; head = lh.y;
+      last = *reinterpret_cast<const int32_t*>(ws.carry + FX_CARRY_SHARPE_LAST);
+    } else {
+      len = st.sh_len[env]; head = st.sh_head[env]; last = st.sh_last_step[env];
+      for (int k = lane; k < Wn; k += 32) ws.ring[k] = gring[k];
+      __syncwarp();
+    }
+    const double ret = (e.equity - e.prev_equity) / c.reward_initial_cash;
+    int slot;  // where the new return lands (same rule as fx_sharpe_push)
+    if (e.bar_index <= last) slot = 0; else slot = (len == Wn) ? head : (head + len) % Wn;
+    const int nn = fx_sharpe_push(ws.ring, 1, Wn, len, head, last, e.bar_index, ret);
+    __syncwarp();
+    r = fx_sharpe_eval_warp(ws.ring, Wn, nn, head, c.annualization_factor, lane);
+    if (lane == 0) {
+      gring[slot] = ret;
+      st.sh_len[env] = len; st.sh_head[env] = head; st.sh_last_step[env] = last;
+      if (CARRY) {
+        *reinterpret_cast<int2*>(ws.carry + FX_CARRY_SHARPE) = make_int2(len, head);
+        *reinterpret_cast<int32_t*>(ws.carry + FX_CARRY_SHARPE_LAST) = last;
+      }
+    }
+  }
+  return r;
+}
+
 // One env-step of one env by one warp (everything between the cross-kernel dependency wait and the release).
 // V: the variant key (FX_V_*).
 // CARRY (fx_rollout_kernel): the step leaves the env's scalar state in ws.carry and returns true if that record is valid;
@@ -828,49 +957,22 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   ts.begin(P, env, lane);
 
   // ---- round trip 1: one batch of independent state loads (invariants: see FxDeviceState)
-  uint32_t flags;
-  int32_t t, total_bars;
-  int64_t start;
-  int n, n_acc;
-  double sub_need;
   FxEnvRegs e;
-  double2 nb_oh, nb_lc;
-  double nb_price, rsv = 0.0;
-  int32_t dec = 0;  // TRUNC: decisions of the episode before this step
+  double rsv = 0.0;
   double prow = 0.0;  // PARAMS: field `lane` of the env's row (lanes 0..6)
   if (PARAMS && lane < FXENV_ENV_PARAMS) prow = fx_env_params(P)[(int64_t)env * FXENV_ENV_PARAMS + lane];
-  if (CARRY && carry_in) {  // the record this warp left behind one step ago (shared memory: broadcast reads)
-    const double* __restrict__ cr = ws.carry;
-    const int2 ft = *reinterpret_cast<const int2*>(cr + FX_CARRY_FLAGS_T);
-    const int2 bn = *reinterpret_cast<const int2*>(cr + FX_CARRY_BARS_N);
-    const int2 at = *reinterpret_cast<const int2*>(cr + FX_CARRY_NACC_TRADES);
-    flags = (uint32_t)ft.x; t = ft.y; total_bars = bn.x; n = bn.y; n_acc = at.x; e.trades = at.y;
-    start = *reinterpret_cast<const long long*>(cr + FX_CARRY_START);
-    sub_need = cr[FX_CARRY_SUBNEED];
-    e.cash = cr[FX_CARRY_CASH]; e.psize = cr[FX_CARRY_PSIZE]; e.pprice = cr[FX_CARRY_PPRICE]; e.equity = cr[FX_CARRY_EQUITY];
-    e.commission_paid = cr[FX_CARRY_COMM];
-    nb_oh.x = cr[FX_CARRY_NBAR]; nb_oh.y = cr[FX_CARRY_NBAR + 1]; nb_lc.x = cr[FX_CARRY_NBAR + 2]; nb_lc.y = cr[FX_CARRY_NBAR + 3];
-    nb_price = cr[FX_CARRY_NBAR + 4];
-    if (TRUNC) dec = *fx_carry_dec(ws);
-    if (lane < FX_RS_N) rsv = cr[FX_CARRY_RSTATS + lane];
-  } else {
-    flags = st.flags[env];
-    t = st.t[env];
-    total_bars = st.total_bars[env];
-    start = st.start[env];
-    n = st.n_orders[env];
-    n_acc = st.n_acc[env];
-    sub_need = st.sub_need[env];
-    e.cash = st.cash[env]; e.psize = st.psize[env]; e.pprice = st.pprice[env]; e.equity = st.equity[env];
-    e.commission_paid = st.commission_paid[env]; e.trades = st.trades[env];
-    // the candle this call works on was saved by the previous call (FxDeviceState::nbar): it travels in this same round trip
-    const double2* __restrict__ nb2 = reinterpret_cast<const double2*>(st.nbar + (int64_t)env * 6);
-    nb_oh = nb2[0]; nb_lc = nb2[1];
-    nb_price = st.nbar[(int64_t)env * 6 + 4];
-    if (TRUNC) dec = P.ep_steps[env];
-    if (lane < FX_RS_N) rsv = st.rstats[(int64_t)env * FX_RS_N + lane];  // DrawDown / TradeAnalyzer / SQN state
-  }
-  e.value = e.equity;
+  FxStepState s0 = fx_step_load<TRUNC, CARRY>(P, env, lane, ws, carry_in, e, rsv);
+  // the step's own copies (the timeline advances flags and t, an auto-reset moves start and total_bars): using the
+  // fields of s0 in their place compiles to different code
+  uint32_t flags = s0.flags;
+  int32_t t = s0.t, total_bars = s0.total_bars;
+  int64_t start = s0.start;
+  int n = s0.n, n_acc = s0.n_acc;
+  double sub_need = s0.sub_need;
+  int32_t dec = s0.dec;
+  double2 nb_oh, nb_lc;
+  nb_oh.x = s0.nb.o; nb_oh.y = s0.nb.h; nb_lc.x = s0.nb.l; nb_lc.y = s0.nb.c;
+  double nb_price = s0.nb_price;
   int action_raw_i = 0;
   float action_raw_f = 0.0f;
   if (!LEAN && c.action_mode == FX_ACTION_CONTINUOUS) action_raw_f = reinterpret_cast<const float*>(actions)[fx_out_idx(o, env)];
@@ -1058,21 +1160,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       fx_mark_to_market<LEAN>(pc, e, b.c);
       // DrawDown analyzer: one notify_fund + next per bar.  With no position and no execution the value is the one of
       // the previous bar and nothing can change.
-      if (any_fill || e.psize != 0.0) {
-        // fx_rs_drawdown in the lane layout: ONE broadcast (the peak), then lanes 0 / 1 / 2 each test their own field;
-        // the percent needs its division only when it can set a new maximum.  The record goes back to memory only when
-        // something in it changed (an execution, a new peak, a new maximum drawdown).
-        const double peak0 = __shfl_sync(FX_FULL, rsv, FX_RS_DD_MAXVALUE);
-        const double peak = e.value > peak0 ? e.value : peak0;
-        const double md = peak - e.value;
-        double cand = (lane == FX_RS_DD_MAXVALUE) ? peak : md;
-        const bool pct_may = (lane == FX_RS_DD_MAX_PCT) && (100.0 * md > rsv * peak * 0.999999);
-        if (__any_sync(FX_FULL, pct_may)) { if (lane == FX_RS_DD_MAX_PCT) cand = pct_may ? 100.0 * md / peak : 0.0; }
-        else if (lane == FX_RS_DD_MAX_PCT) cand = 0.0;
-        const bool up = (lane <= FX_RS_DD_MAX_PCT) && (cand > rsv);
-        if (up) rsv = cand;
-        if (any_fill || __any_sync(FX_FULL, up)) { if (lane < FX_RS_N) st.rstats[(int64_t)env * FX_RS_N + lane] = rsv; }
-      }
+      fx_step_drawdown(st, env, lane, e, any_fill, rsv);
     }
     ts.at(lane, 5);  // broker pass done, marked to market
     // candle of the next call (lanes 0..4): requested now, stored at the end of the env-step
@@ -1144,42 +1232,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
     ts.at(lane, 6);  // strategy + publish
 
     // ---- reward plugin (app/env.py:148-155)
-    if (REWARD == FX_REWARD_PNL) {
-      r = fx_reward_pnl(c, e);
-    } else if (REWARD == FX_REWARD_DD) {
-      double peak = st.dd_peak[env];
-      int32_t last = st.dd_last_step[env];
-      r = fx_reward_dd(c, e, peak, last);
-      if (lane == 0) { st.dd_peak[env] = peak; st.dd_last_step[env] = last; }
-    } else {
-      // deque of per-step returns: stage the ring in shared memory (coalesced), push, evaluate in Python order
-      const int Wn = c.sharpe_window;
-      double* gring = st.sh_ring + (int64_t)env * Wn;
-      int32_t len, head, last;
-      if (CARRY && carry_in) {  // this warp ran the env's previous step: its copy of the deque is current
-        const int2 lh = *reinterpret_cast<const int2*>(ws.carry + FX_CARRY_SHARPE);
-        len = lh.x; head = lh.y;
-        last = *reinterpret_cast<const int32_t*>(ws.carry + FX_CARRY_SHARPE_LAST);
-      } else {
-        len = st.sh_len[env]; head = st.sh_head[env]; last = st.sh_last_step[env];
-        for (int k = lane; k < Wn; k += 32) ws.ring[k] = gring[k];
-        __syncwarp();
-      }
-      const double ret = (e.equity - e.prev_equity) / c.reward_initial_cash;
-      int slot;  // where the new return lands (same rule as fx_sharpe_push)
-      if (e.bar_index <= last) slot = 0; else slot = (len == Wn) ? head : (head + len) % Wn;
-      const int nn = fx_sharpe_push(ws.ring, 1, Wn, len, head, last, e.bar_index, ret);
-      __syncwarp();
-      r = fx_sharpe_eval_warp(ws.ring, Wn, nn, head, c.annualization_factor, lane);
-      if (lane == 0) {
-        gring[slot] = ret;
-        st.sh_len[env] = len; st.sh_head[env] = head; st.sh_last_step[env] = last;
-        if (CARRY) {
-          *reinterpret_cast<int2*>(ws.carry + FX_CARRY_SHARPE) = make_int2(len, head);
-          *reinterpret_cast<int32_t*>(ws.carry + FX_CARRY_SHARPE_LAST) = last;
-        }
-      }
-    }
+    r = fx_step_reward<REWARD, CARRY>(P, e, env, lane, ws, carry_in);
     const bool term = ((e.flags & FX_FLAG_TERMINATED) != 0u) || (e.equity <= c.min_equity);  // app/env.py:157
     bool trunc = TRUNC && (e.flags & FX_FLAG_TRUNCATED) != 0u;  // the window ran out (FXENV_TIME_LIMIT_WINDOW)
     if (REPEAT) {  // the step's reward: the substeps' sum in substep order, from r0; a terminating substep ends the step
