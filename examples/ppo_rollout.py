@@ -13,6 +13,7 @@ minibatch and advantages are normalised with global statistics (gym_fx_b200.lear
     python examples/ppo_rollout.py --envs 4096 --episode-bars 500 --holdout-frac 0.2 --eval-rollouts 2
     python examples/ppo_rollout.py --envs 4096 --action-repeat 5 --repeat-mode hold
     python examples/ppo_rollout.py --hidden 64
+    python examples/ppo_rollout.py --separate-critic --updates 5
     python examples/ppo_rollout.py --randomize-costs 1e-4,3e-4
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 examples/ppo_rollout.py --envs 4096
 
@@ -74,6 +75,8 @@ def main():
                     help="repeat: the action on every bar of a step; hold: on its first bar, then hold")
     ap.add_argument("--hidden", type=int, choices=(64, 128, 256, 512), default=256,
                     help="width of both hidden layers of the actor-critic")
+    ap.add_argument("--separate-critic", action="store_true",
+                    help="separate actor and critic networks of width --hidden instead of one shared body")
     ap.add_argument("--max-episode-steps", type=int, default=0,
                     help="time limit: an episode is truncated after this many decisions (0: none)")
     ap.add_argument("--truncate-window", action="store_true",
@@ -160,7 +163,7 @@ def main():
 
     torch.backends.cuda.matmul.allow_tf32 = True
     torch.manual_seed(0)  # identical replicas on every rank
-    net = ActorCritic(D, hidden=args.hidden, continuous=continuous).to(dev)
+    net = ActorCritic(D, hidden=args.hidden, continuous=continuous, separate=args.separate_critic).to(dev)
     opt = torch.optim.Adam(net.parameters(), lr=args.lr, eps=1e-5)
     policy = env.make_policy(net)
     buf = None
@@ -234,9 +237,10 @@ def main():
         steps = N * world * H * n_it
         print(json.dumps({
             "example": "ppo_rollout", "workload": desc, "n_gpus": world, "envs_per_gpu": N, "horizon": H,
-            "policy": f"MLP({D},{args.hidden},{args.hidden}) actor-critic ({args.action_space} actions), fused wgmma kernel in the rollout, "
+            "policy": f"MLP({D},{args.hidden},{args.hidden}) actor-critic, {'separate actor and critic' if args.separate_critic else 'shared body'} "
+                      f"({args.action_space} actions), fused wgmma kernel in the rollout, "
                       "torch (tf32) in the update",
-            "hidden": args.hidden, "rollout_env_steps_per_s": steps / max(t_roll, 1e-9), "rollout_us_per_step": t_roll / (H * n_it) * 1e6,
+            "hidden": args.hidden, "separate_critic": args.separate_critic, "rollout_env_steps_per_s": steps / max(t_roll, 1e-9), "rollout_us_per_step": t_roll / (H * n_it) * 1e6,
             "action_repeat": K, "repeat_mode": args.repeat_mode, "randomize_costs": list(cost_max) if cost_max else None,
             "rollout_bars_per_s_upper_bound": steps * K / max(t_roll, 1e-9),
             "train_env_steps_per_s": steps / max(t_roll + t_upd, 1e-9), "update_s": t_upd / n_it, **stats}), flush=True)

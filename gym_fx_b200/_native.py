@@ -32,13 +32,14 @@ EXPORTS = [
     "fxenv_policy_create", "fxenv_policy_set_weights", "fxenv_policy_destroy", "fxenv_rollout", "fxenv_policy_sync_timeouts",
     "fxenv_rollout_ex", "fxenv_policy_peek", "fxenv_set_reset_starts", "fxenv_get_episode_info",
     "fxenv_set_bracket_audit", "fxenv_get_bracket_audit", "fxenv_set_action_repeat", "fxenv_policy_create_ex",
-    "fxenv_set_time_limit", "fxenv_set_env_params",
+    "fxenv_set_time_limit", "fxenv_set_env_params", "fxenv_policy_create_ex2",
 ]
 
 ROLLOUT_GREEDY = 1  # FXENV_ROLLOUT_GREEDY
 PEEK_OBS16, PEEK_H1 = 0, 1  # FXENV_PEEK_*
 MAX_REPEAT, REPEAT_HOLD = 256, 1  # FXENV_MAX_REPEAT, FXENV_REPEAT_HOLD
 POLICY_WIDTHS = (64, 128, 256, 512)  # the hidden widths fxenv_policy_create_ex accepts
+POLICY_SEPARATE = 1  # FXENV_POLICY_SEPARATE (fxenv_policy_create_ex2 flags)
 FLAG_TRUNCATED, TIME_LIMIT_WINDOW = 64, 1  # FX_FLAG_TRUNCATED, FXENV_TIME_LIMIT_WINDOW
 DONE_TERMINATED, DONE_TRUNCATED = 1, 2  # FXENV_DONE_* codes of the terminated / done outputs while truncation is on
 # FXENV_ENV_PARAMS and the FXENV_PARAM_* columns of a per-env parameter row (fxenv_set_env_params)
@@ -139,6 +140,7 @@ def load():
     L.fxenv_step_many_engine.argtypes = [vp, C.c_int]
     L.fxenv_policy_create.argtypes = [vp, C.POINTER(vp)]
     L.fxenv_policy_create_ex.argtypes = [vp, C.c_int32, C.POINTER(vp)]
+    L.fxenv_policy_create_ex2.argtypes = [vp, C.c_int32, C.c_uint32, C.POINTER(vp)]
     L.fxenv_policy_set_weights.argtypes = [vp, C.POINTER(FxPolicyWeights), vp]
     L.fxenv_policy_destroy.argtypes = [vp]
     L.fxenv_rollout.argtypes = [vp, vp, C.POINTER(FxRollout), vp]

@@ -826,12 +826,14 @@ struct FxPolicy {
   FxEnv* env = nullptr;
   int k_pad = 0;                       // obs_dim padded to a multiple of 64 (bf16 row stride of the observation copy)
   int hidden = FX_POLICY_HIDDEN;       // width of both hidden layers: 64, 128, 256 or 512 (fxenv_policy_create_ex)
-  uint16_t* w1 = nullptr;              // bf16 [hidden][k_pad]
-  uint16_t* w2 = nullptr;              // bf16 [hidden][hidden]
-  float* fparams = nullptr;            // b1[hidden] | b2[hidden] | head_w[4][hidden] | head_b[4]
+  bool separate = false;               // FXENV_POLICY_SEPARATE: actor and critic trunks, stacked (nets = 2) below
+  int nets = 1;                        // trunks: 1 (shared body) or 2 (actor, critic)
+  uint16_t* w1 = nullptr;              // bf16 [nets][hidden][k_pad]
+  uint16_t* w2 = nullptr;              // bf16 [nets][hidden][hidden]
+  float* fparams = nullptr;            // b1[nets][hidden] | b2[nets][hidden] | head_w[4][hidden] | head_b[4]
   uint16_t* obs16[2] = {nullptr, nullptr};  // bf16 [num_envs][k_pad], double buffered
-  uint16_t* h1 = nullptr;              // bf16 [num_envs padded to whole tiles][hidden]: the two halves of h1 meet here
-  float* head_part = nullptr;          // float4 [num_envs padded]: partial head sums of the second CTA of a pair
+  uint16_t* h1 = nullptr;              // bf16 [num_envs padded to whole tiles][nets * hidden]: where the halves meet
+  float* head_part = nullptr;          // float4 [num_envs padded][nets]: partial head sums of the second CTA of a pair
   int32_t* sync = nullptr;             // act_flag[tiles] | done_cnt[tiles] | timeouts[1] (FxTileSync), zeroed per rollout
   int tiles = 0;
   int32_t* scratch_act = nullptr;      // bootstrap evaluation: action / logp are discarded
@@ -889,8 +891,9 @@ cudaError_t enqueue_rollout(FxEnv* env, FxPolicy* pol, const FxRollout& io, uint
                                                                           // 1 = no env steps, 2 = no policy evaluations
   // FXENV_TILE_SYNC=1: per-tile hand-over between the two kernels (FxTileSync) instead of whole-kernel dependencies.
   // Off by default: bit-identical results, but the kernel boundary it removes is paid back by the polling warps.
+  // A separate actor and critic always runs in kernel order: the actor pair's flag does not cover the critic pair.
   const char* tsv = getenv("FXENV_TILE_SYNC");
-  const bool tile_sync = !skip && tsv && atoi(tsv) != 0;
+  const bool tile_sync = !skip && !pol->separate && tsv && atoi(tsv) != 0;
   cudaError_t e = cudaMemsetAsync(pol->sync, 0, (2 * (size_t)pol->tiles + 1) * sizeof(int32_t), s);
   if (e != cudaSuccess) return e;
   e = fx_launch_observe(env->P, io.obs, s, pol->obs16[0], pol->k_pad);  // the current observation, both copies
@@ -919,7 +922,7 @@ cudaError_t enqueue_rollout(FxEnv* env, FxPolicy* pol, const FxRollout& io, uint
                            (!last && io.gumbel) ? io.gumbel + (size_t)t * N * noise_per_env : nullptr, io.seed, (unsigned)t,
                            last ? static_cast<void*>(pol->scratch_act) : actions + (size_t)t * N,
                            last ? pol->scratch_logp : io.logp + (size_t)t * N, io.value + (size_t)t * N, sg, (int)e0, (int)e1,
-                           tile_sync, pol->continuous, greedy);
+                           tile_sync, pol->continuous, greedy, pol->separate);
       if (e != cudaSuccess) return e;
       if (last) break;
       const FxTileSync ts = {pol->dev.act_flag, pol->sync + pol->tiles, pol->dev.timeouts, t + 1};
@@ -977,7 +980,7 @@ int64_t fxenv_policy_peek(FxPolicy* pol, int what, int slot, void* dst, int64_t 
     n = (int64_t)env->P.cfg.num_envs * pol->k_pad * 2;
   } else if (what == FXENV_PEEK_H1 && slot == 0) {
     src = pol->h1;
-    n = (int64_t)pol->tiles * FX_POLICY_TILE_M * pol->hidden * 2;
+    n = (int64_t)pol->tiles * FX_POLICY_TILE_M * pol->nets * pol->hidden * 2;
   } else {
     return fail(env, FXENV_E_INVALID, "fxenv_policy_peek: unknown buffer or slot");
   }
@@ -993,8 +996,13 @@ int fxenv_policy_create(FxEnv* env, FxPolicy** out) {
 }
 
 int fxenv_policy_create_ex(FxEnv* env, int32_t hidden, FxPolicy** out) {
+  return fxenv_policy_create_ex2(env, hidden, 0u, out);
+}
+
+int fxenv_policy_create_ex2(FxEnv* env, int32_t hidden, uint32_t flags, FxPolicy** out) {
   if (!env || !out) return FXENV_E_INVALID;
   *out = nullptr;
+  if (flags & ~(uint32_t)FXENV_POLICY_SEPARATE) return fail(env, FXENV_E_INVALID, "unknown policy flags");
   if (env->P.cfg.action_mode != FX_ACTION_DISCRETE && env->P.cfg.action_mode != FX_ACTION_CONTINUOUS)
     return fail(env, FXENV_E_INVALID, "unknown action mode");
   if (!fx_policy_width_ok(hidden))
@@ -1005,32 +1013,35 @@ int fxenv_policy_create_ex(FxEnv* env, int32_t hidden, FxPolicy** out) {
   pol->env = env;
   pol->continuous = env->P.cfg.action_mode == FX_ACTION_CONTINUOUS;
   pol->hidden = hidden;
+  pol->separate = (flags & FXENV_POLICY_SEPARATE) != 0;
+  pol->nets = pol->separate ? 2 : 1;
   const size_t N = (size_t)env->P.cfg.num_envs, D = (size_t)env->P.obs_dim;
   pol->k_pad = (int)((D + 63) / 64 * 64);
-  const size_t KP = (size_t)pol->k_pad, Hd = (size_t)hidden;
-  bool ok = cudaMalloc(&pol->w1, Hd * KP * 2) == cudaSuccess && cudaMalloc(&pol->w2, Hd * Hd * 2) == cudaSuccess &&
-            cudaMalloc(&pol->fparams, (2 * Hd + 4 * Hd + 4) * sizeof(float)) == cudaSuccess &&
+  const size_t KP = (size_t)pol->k_pad, Hd = (size_t)hidden, Hn = (size_t)pol->nets * Hd;  // Hn: stacked trunk rows
+  bool ok = cudaMalloc(&pol->w1, Hn * KP * 2) == cudaSuccess && cudaMalloc(&pol->w2, Hn * Hd * 2) == cudaSuccess &&
+            cudaMalloc(&pol->fparams, (2 * Hn + 4 * Hd + 4) * sizeof(float)) == cudaSuccess &&
             cudaMalloc(&pol->obs16[0], N * KP * 2) == cudaSuccess && cudaMalloc(&pol->obs16[1], N * KP * 2) == cudaSuccess &&
             cudaMalloc(&pol->scratch_act, N * 4) == cudaSuccess && cudaMalloc(&pol->scratch_logp, N * 4) == cudaSuccess;
   const size_t NP = (N + FX_POLICY_TILE_M - 1) / FX_POLICY_TILE_M * FX_POLICY_TILE_M;  // whole 128-env tiles
-  ok = ok && cudaMalloc(&pol->h1, NP * Hd * 2) == cudaSuccess && cudaMalloc(&pol->head_part, NP * 4 * sizeof(float)) == cudaSuccess;
+  ok = ok && cudaMalloc(&pol->h1, NP * Hn * 2) == cudaSuccess &&
+       cudaMalloc(&pol->head_part, NP * pol->nets * 4 * sizeof(float)) == cudaSuccess;
   pol->tiles = (int)(NP / FX_POLICY_TILE_M);
   ok = ok && cudaMalloc(&pol->sync, (2 * (size_t)pol->tiles + 1) * sizeof(int32_t)) == cudaSuccess;
   if (!ok) { fxenv_policy_destroy(pol); return fail(env, FXENV_E_CUDA, "cudaMalloc(policy buffers) failed"); }
   // the K padding of the observation copies is never written by the env kernels: zero it once
   cudaMemset(pol->obs16[0], 0, N * KP * 2);
   cudaMemset(pol->obs16[1], 0, N * KP * 2);
-  pol->dev.b1 = pol->fparams; pol->dev.b2 = pol->fparams + Hd; pol->dev.head_w = pol->fparams + 2 * Hd;
-  pol->dev.head_b = pol->fparams + 6 * Hd;
+  pol->dev.b1 = pol->fparams; pol->dev.b2 = pol->fparams + Hn; pol->dev.head_w = pol->fparams + 2 * Hn;
+  pol->dev.head_b = pol->fparams + 2 * Hn + 4 * Hd;
   pol->dev.h1 = pol->h1; pol->dev.head_part = reinterpret_cast<float4*>(pol->head_part);
   pol->dev.dbg = env->P.timeline;  // (nullptr unless FXENV_TIMELINE is set; only the timing build looks at it)
   pol->dev.act_flag = pol->sync; pol->dev.done_cnt = pol->sync + pol->tiles; pol->dev.timeouts = pol->sync + 2 * pol->tiles;
   cudaMemset(pol->sync, 0, (2 * (size_t)pol->tiles + 1) * sizeof(int32_t));
   int rc = make_map(env, &pol->map_obs[0], pol->obs16[0], N, KP, FX_POLICY_TILE_M);
   if (!rc) rc = make_map(env, &pol->map_obs[1], pol->obs16[1], N, KP, FX_POLICY_TILE_M);
-  if (!rc) rc = make_map(env, &pol->map_w1, pol->w1, Hd, KP, (uint32_t)Hd / 2);   // a CTA loads its half of the units
-  if (!rc) rc = make_map(env, &pol->map_w2, pol->w2, Hd, Hd, (uint32_t)Hd / 2);
-  if (!rc) rc = make_map(env, &pol->map_h1, pol->h1, NP, Hd, FX_POLICY_TILE_M);
+  if (!rc) rc = make_map(env, &pol->map_w1, pol->w1, Hn, KP, (uint32_t)Hd / 2);   // a CTA loads its half of the units
+  if (!rc) rc = make_map(env, &pol->map_w2, pol->w2, Hn, Hd, (uint32_t)Hd / 2);
+  if (!rc) rc = make_map(env, &pol->map_h1, pol->h1, NP, Hn, FX_POLICY_TILE_M);
   if (rc) { fxenv_policy_destroy(pol); return rc; }
   cudaError_t ce = fx_policy_configure();
   for (auto& st : pol->side) if (ce == cudaSuccess) ce = cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
@@ -1047,23 +1058,25 @@ int fxenv_policy_set_weights(FxPolicy* pol, const FxPolicyWeights* w, void* stre
   if (!w->w1 || !w->b1 || !w->w2 || !w->b2 || !w->w_pi || !w->b_pi || !w->w_v || !w->b_v) return fail(env, FXENV_E_INVALID, "null weight pointer");
   DeviceGuard g(env->device);
   cudaStream_t s = (cudaStream_t)stream_;
-  const int D = env->P.obs_dim, Hd = pol->hidden;
-  FX_CUDA(env, fx_policy_pack(w->w1, pol->w1, Hd, D, pol->k_pad, s));
-  FX_CUDA(env, fx_policy_pack(w->w2, pol->w2, Hd, Hd, Hd, s));
+  const int D = env->P.obs_dim, Hd = pol->hidden, Hn = pol->nets * Hd;  // Hn: stacked trunk rows
+  FX_CUDA(env, fx_policy_pack(w->w1, pol->w1, Hn, D, pol->k_pad, s));
+  FX_CUDA(env, fx_policy_pack(w->w2, pol->w2, Hn, Hd, Hd, s));
   float* f = pol->fparams;
-  FX_CUDA(env, cudaMemcpyAsync(f, w->b1, Hd * 4, cudaMemcpyDeviceToDevice, s));
-  FX_CUDA(env, cudaMemcpyAsync(f + Hd, w->b2, Hd * 4, cudaMemcpyDeviceToDevice, s));
+  float* hw = f + 2 * Hn;      // head rows [4][Hd]
+  float* hb = hw + 4 * Hd;     // head bias [4]
+  FX_CUDA(env, cudaMemcpyAsync(f, w->b1, Hn * 4, cudaMemcpyDeviceToDevice, s));
+  FX_CUDA(env, cudaMemcpyAsync(f + Hn, w->b2, Hn * 4, cudaMemcpyDeviceToDevice, s));
   if (pol->continuous) {  // head rows {w_mu, 0, 0, w_v}, head bias {b_mu, log sigma, 0, b_v}
-    FX_CUDA(env, cudaMemcpyAsync(f + 2 * Hd, w->w_pi, Hd * 4, cudaMemcpyDeviceToDevice, s));
-    FX_CUDA(env, cudaMemsetAsync(f + 3 * Hd, 0, 2 * Hd * 4, s));
-    FX_CUDA(env, cudaMemcpyAsync(f + 6 * Hd, w->b_pi, 2 * 4, cudaMemcpyDeviceToDevice, s));
-    FX_CUDA(env, cudaMemsetAsync(f + 6 * Hd + 2, 0, 4, s));
+    FX_CUDA(env, cudaMemcpyAsync(hw, w->w_pi, Hd * 4, cudaMemcpyDeviceToDevice, s));
+    FX_CUDA(env, cudaMemsetAsync(hw + Hd, 0, 2 * Hd * 4, s));
+    FX_CUDA(env, cudaMemcpyAsync(hb, w->b_pi, 2 * 4, cudaMemcpyDeviceToDevice, s));
+    FX_CUDA(env, cudaMemsetAsync(hb + 2, 0, 4, s));
   } else {
-    FX_CUDA(env, cudaMemcpyAsync(f + 2 * Hd, w->w_pi, 3 * Hd * 4, cudaMemcpyDeviceToDevice, s));
-    FX_CUDA(env, cudaMemcpyAsync(f + 6 * Hd, w->b_pi, 3 * 4, cudaMemcpyDeviceToDevice, s));
+    FX_CUDA(env, cudaMemcpyAsync(hw, w->w_pi, 3 * Hd * 4, cudaMemcpyDeviceToDevice, s));
+    FX_CUDA(env, cudaMemcpyAsync(hb, w->b_pi, 3 * 4, cudaMemcpyDeviceToDevice, s));
   }
-  FX_CUDA(env, cudaMemcpyAsync(f + 5 * Hd, w->w_v, Hd * 4, cudaMemcpyDeviceToDevice, s));
-  FX_CUDA(env, cudaMemcpyAsync(f + 6 * Hd + 3, w->b_v, 4, cudaMemcpyDeviceToDevice, s));
+  FX_CUDA(env, cudaMemcpyAsync(hw + 3 * Hd, w->w_v, Hd * 4, cudaMemcpyDeviceToDevice, s));
+  FX_CUDA(env, cudaMemcpyAsync(hb + 3, w->b_v, 4, cudaMemcpyDeviceToDevice, s));
   env->launches += 2;
   pol->has_weights = true;
   return FXENV_OK;

@@ -34,6 +34,14 @@
 // Other widths change only the N of the MMAs (HID / 2), the accumulators per thread (HID / 4), the W1 / W2 tile rows,
 // the layer-2 k-blocks (HID / 64), the h1 row stride and the head loops; at 512 the eight layer-2 k-blocks outrun the
 // 4-stage ring, so the later ones are streamed after the cluster barrier (kRefill2), and the kernel runs one CTA per SM.
+//
+// Separate actor and critic networks (the template parameter SEP): two CTA pairs per tile, blockIdx.x = 4 tile + 2 net
+// + rank, net 0 = the actor, 1 = the critic.  Each pair is the kernel above at width HID over its own network's rows
+// of the stacked parameters (W1 [2 HID][KP], W2 [2 HID][HID], b1 / b2 [2 HID], actor first; h1 [rows][2 HID], the
+// network's HID columns at net HID).  The pairs never talk to each other: the actor pair samples from head rows 0-2
+// and stores action / log-prob, the critic pair stores the value of row 3; head_part holds one float4 per row and
+// network.  No per-tile hand-over: the actor pair's act_flag would not cover the critic pair's reads of the
+// observation slot.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -201,7 +209,8 @@ constexpr float kHalfLog2Pi = 0.918938533204672742f;
 // HID: hidden units of both layers (64, 128, 256 or 512).
 // CONT = false: discrete actions (int32, Gumbel-max over 3 logits; noise: float32 [num_envs][3] Gumbel(0,1)).
 // CONT = true:  continuous actions (float32, Gaussian; noise: float32 [num_envs] N(0,1)).
-template <int HID, bool CONT>
+// SEP = true:   separate actor and critic networks, two CTA pairs per tile (see the top of the file).
+template <int HID, bool CONT, bool SEP>
 __global__ void __launch_bounds__(kThreads, Width<HID>::kMinBlocks)
 fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_constant__ CUtensorMap map_w1,
                  const __grid_constant__ CUtensorMap map_w2, const __grid_constant__ CUtensorMap map_h1, const FxPolicyDev pol,
@@ -218,8 +227,15 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
   float* bias = reinterpret_cast<float*>(smem + kOffBias);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = blockIdx.x & 1;                         // which half of the hidden units (cluster = CTA pair)
-  const int m0 = env_begin + (blockIdx.x >> 1) * kTileM;   // a launch covers the envs [env_begin, num_envs) (env groups)
+  const int m0 = env_begin + (blockIdx.x >> (SEP ? 2 : 1)) * kTileM;  // a launch covers the envs [env_begin, num_envs)
   const int n0 = rank * kHalfN;
+  // SEP: which network this pair computes; its rows of W1 / W2 / b1 / b2 and its columns of h1 start at net * HID
+  const int net = SEP ? (int)(blockIdx.x >> 1) & 1 : 0;
+  const int wrow = net * HID + n0;                         // this CTA's first row of W1 / W2, first column of h1
+  constexpr int kH1Cols = SEP ? 2 * HID : HID;             // h1 row stride
+  constexpr int kParts = SEP ? 2 : 1;                      // head_part float4s per row
+  const bool actor = !SEP || net == 0, critic = !SEP || net == 1;
+  const bool tsync = !SEP && tile_sync;
   const bool producer = warp == kConsumerWarps;
 #ifdef FXENV_ENABLE_TIMING  // kernel-chain probe (tools/chain_probe.py): CTA 0 logs {kind, entry, after the wait, exit}
   long long* klog = nullptr;
@@ -242,7 +258,7 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
   // small fp32 parameters (weights of this launch, not produced by the previous kernel): plain loads
   for (int i = threadIdx.x; i < 4 * HID; i += kThreads) head_w[i] = pol.head_w[i];
   for (int i = threadIdx.x; i < 2 * HID + 4; i += kThreads)
-    bias[i] = (i < HID) ? pol.b1[i] : (i < 2 * HID ? pol.b2[i - HID] : pol.head_b[i - 2 * HID]);
+    bias[i] = (i < HID) ? pol.b1[net * HID + i] : (i < 2 * HID ? pol.b2[net * HID + i - HID] : pol.head_b[i - 2 * HID]);
   __syncthreads();
   asm volatile("griddepcontrol.launch_dependents;");  // the env step that consumes our actions may get scheduled early
   const int kb2 = HID / kBlockK;             // k-blocks of layer 2 (1, 2, 4, 8)
@@ -268,9 +284,9 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
         unsigned char* st = smem + it * kStageBytes;
         const bool l1 = it < k_blocks1;
         mbar_expect_tx(&bar->full[it], kStageBytes);
-        tma_load_2d(l1 ? &map_w1 : &map_w2, &bar->full[it], st + kABytes, (l1 ? it : it - k_blocks1) * kBlockK, n0);
+        tma_load_2d(l1 ? &map_w1 : &map_w2, &bar->full[it], st + kABytes, (l1 ? it : it - k_blocks1) * kBlockK, wrow);
       }
-      if (tile_sync && step > 0u) {
+      if (tsync && step > 0u) {
         // closed loop: this tile's rows are complete once its envs have finished step - 1 (counted by the step kernel,
         // which is resident with us: see FxTileSync) -- no need to wait for the whole step grid to drain
         const int valid = (num_envs - m0 < kTileM) ? num_envs - m0 : kTileM;
@@ -296,7 +312,7 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
         if (it >= kStages) {
           mbar_wait(&bar->empty[s], ((it / kStages) - 1) & 1);
           mbar_expect_tx(&bar->full[s], kStageBytes);
-          tma_load_2d(l1 ? &map_w1 : &map_w2, &bar->full[s], st + kABytes, (l1 ? it : it - k_blocks1) * kBlockK, n0);
+          tma_load_2d(l1 ? &map_w1 : &map_w2, &bar->full[s], st + kABytes, (l1 ? it : it - k_blocks1) * kBlockK, wrow);
         }
         if (l1) tma_load_2d(&map_obs, &bar->full[s], st, it * kBlockK, m0);
         // (layer 2: the W2 tile is in flight; the h1 tile of the same stage follows in phase 2)
@@ -313,8 +329,8 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
       if (lane == 0) mbar_arrive(&bar->empty[s]);
     }
     const float* b1 = bias + n0;
-    uint32_t* h_lo = reinterpret_cast<uint32_t*>(pol.h1 + (size_t)(m0 + r_lo) * HID + n0 + c_lane);
-    uint32_t* h_hi = h_lo + 8 * HID / 2;
+    uint32_t* h_lo = reinterpret_cast<uint32_t*>(pol.h1 + (size_t)(m0 + r_lo) * kH1Cols + wrow + c_lane);
+    uint32_t* h_hi = h_lo + 8 * kH1Cols / 2;
 #pragma unroll
     for (int j = 0; j < kAcc / 4; j++) {
       const float bb0 = b1[8 * j + c_lane], bb1 = b1[8 * j + c_lane + 1];
@@ -337,9 +353,9 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
         if (kRefill2 && j >= kStages) {  // (HID = 512: the W2 tile of a stage past the ring, once its slot is free)
           mbar_wait(&bar->empty[s], ((it / kStages) - 1) & 1);
           mbar_expect_tx(&bar->full[s], kStageBytes);
-          tma_load_2d(&map_w2, &bar->full[s], smem + s * kStageBytes + kABytes, j * kBlockK, n0);
+          tma_load_2d(&map_w2, &bar->full[s], smem + s * kStageBytes + kABytes, j * kBlockK, wrow);
         }
-        tma_load_2d(&map_h1, &bar->full[s], smem + s * kStageBytes, j * kBlockK, m0);
+        tma_load_2d(&map_h1, &bar->full[s], smem + s * kStageBytes, net * HID + j * kBlockK, m0);
       }
     }
   } else {
@@ -350,6 +366,8 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
       if (kRefill2 && j + kStages < kb2 && lane == 0) mbar_arrive(&bar->empty[s]);  // the slot takes k-block j + 4
     }
     const float* b2 = bias + HID + n0;
+    // (SEP: both pairs reduce all four rows and each stores only its own; skipping the other network's rows takes a
+    // copy of this unrolled loop per network, which at HID = 256 and 512 spills past the register cap)
 #pragma unroll
     for (int i = 0; i < kAcc; i++) {
       const int k = n0 + 8 * (i / 4) + c_lane + (i & 1);
@@ -371,8 +389,8 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
       acc_hi[q] += __shfl_xor_sync(0xffffffffu, acc_hi[q], 2);
     }
     if (rank == 1 && (lane & 3) == 0) {
-      pol.head_part[m0 + r_lo] = make_float4(acc_lo[0], acc_lo[1], acc_lo[2], acc_lo[3]);
-      pol.head_part[m0 + r_lo + 8] = make_float4(acc_hi[0], acc_hi[1], acc_hi[2], acc_hi[3]);
+      pol.head_part[(m0 + r_lo) * kParts + net] = make_float4(acc_lo[0], acc_lo[1], acc_lo[2], acc_lo[3]);
+      pol.head_part[(m0 + r_lo + 8) * kParts + net] = make_float4(acc_hi[0], acc_hi[1], acc_hi[2], acc_hi[3]);
     }
   }
   cluster_sync();  // rank 1's partial head sums are visible to rank 0
@@ -382,10 +400,11 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
       const int env = m0 + r_lo + 8 * half;
       const float* acc = half ? acc_hi : acc_lo;
       if ((lane & 3) == 0 && env < num_envs) {
-        const float4 o = pol.head_part[env];
+        const float4 o = pol.head_part[env * kParts + net];
         const float* hb = bias + 2 * HID;
         // (rank 0's columns first, then rank 1's: a fixed order, so the result does not depend on timing)
-        if (CONT) {
+        // (SEP: the actor pair samples and stores action / log-prob, the critic pair stores the value)
+        if (actor && CONT) {
           const float mu = (acc[0] + o.x) + hb[0], log_std = hb[1];
           float eps = 0.f;  // greedy: the mean
           if (!greedy) {
@@ -398,7 +417,7 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
           }
           reinterpret_cast<float*>(action_)[env] = fmaf(expf(log_std), eps, mu);
           logp[env] = (-0.5f * eps * eps - log_std) - kHalfLog2Pi;
-        } else {
+        } else if (actor) {
           const float l0 = (acc[0] + o.x) + hb[0], l1 = (acc[1] + o.y) + hb[1], l2 = (acc[2] + o.z) + hb[2];
           float g0 = 0.f, g1 = 0.f, g2 = 0.f;  // greedy: the argmax of the logits
           if (!greedy) {
@@ -418,10 +437,10 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
           reinterpret_cast<int32_t*>(action_)[env] = a;
           logp[env] = (a == 0 ? l0 : (a == 1 ? l1 : l2)) - lse;
         }
-        value[env] = (acc[3] + o.w) + hb[3];
+        if (critic) value[env] = (acc[3] + o.w) + hb[3];
       }
     }
-    if (tile_sync) {  // the tile's actions are stored: the step kernel's warps of these envs may go
+    if (tsync) {  // the tile's actions are stored: the step kernel's warps of these envs may go
       asm volatile("bar.sync 1, %0;" :: "n"(kConsumerThreads) : "memory");  // the two consumer warpgroups
       if (threadIdx.x == 0) {
         __threadfence();
@@ -443,18 +462,24 @@ __global__ void fx_policy_pack_kernel(const float* __restrict__ src, uint16_t* _
   dst[i] = c < cols ? __bfloat16_as_ushort(__float2bfloat16_rn(src[(int64_t)r * cols + c])) : (uint16_t)0;
 }
 
-using PolicyKernel = decltype(&fx_policy_kernel<256, false>);
+using PolicyKernel = decltype(&fx_policy_kernel<256, false, false>);
 
-// the instantiation of one width and action mode, with its dynamic shared memory; nullptr for an unsupported width
-template <bool CONT>
+// the instantiation of one width, action mode and network layout, with its dynamic shared memory; nullptr for an
+// unsupported width
+template <bool CONT, bool SEP>
 PolicyKernel policy_kernel(int hidden, uint32_t* smem) {
   switch (hidden) {
-    case 64: *smem = Width<64>::kSmemBytes; return fx_policy_kernel<64, CONT>;
-    case 128: *smem = Width<128>::kSmemBytes; return fx_policy_kernel<128, CONT>;
-    case 256: *smem = Width<256>::kSmemBytes; return fx_policy_kernel<256, CONT>;
-    case 512: *smem = Width<512>::kSmemBytes; return fx_policy_kernel<512, CONT>;
+    case 64: *smem = Width<64>::kSmemBytes; return fx_policy_kernel<64, CONT, SEP>;
+    case 128: *smem = Width<128>::kSmemBytes; return fx_policy_kernel<128, CONT, SEP>;
+    case 256: *smem = Width<256>::kSmemBytes; return fx_policy_kernel<256, CONT, SEP>;
+    case 512: *smem = Width<512>::kSmemBytes; return fx_policy_kernel<512, CONT, SEP>;
     default: *smem = 0; return nullptr;
   }
+}
+
+PolicyKernel policy_kernel(int hidden, bool continuous, bool separate, uint32_t* smem) {
+  if (separate) return continuous ? policy_kernel<true, true>(hidden, smem) : policy_kernel<false, true>(hidden, smem);
+  return continuous ? policy_kernel<true, false>(hidden, smem) : policy_kernel<false, false>(hidden, smem);
 }
 
 }  // namespace
@@ -469,18 +494,19 @@ bool fx_policy_width_ok(int hidden) { return hidden == 64 || hidden == 128 || hi
 
 size_t fx_policy_smem_bytes(int hidden) {
   uint32_t smem = 0;
-  policy_kernel<false>(hidden, &smem);
+  policy_kernel<false, false>(hidden, &smem);
   return smem;
 }
 
 cudaError_t fx_policy_configure() {
   for (int hidden : {64, 128, 256, 512})
-    for (bool cont : {false, true}) {
-      uint32_t smem = 0;
-      PolicyKernel k = cont ? policy_kernel<true>(hidden, &smem) : policy_kernel<false>(hidden, &smem);
-      cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) return e;
-    }
+    for (bool cont : {false, true})
+      for (bool sep : {false, true}) {
+        uint32_t smem = 0;
+        PolicyKernel k = policy_kernel(hidden, cont, sep, &smem);
+        cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return e;
+      }
   return cudaSuccess;
 }
 
@@ -488,13 +514,15 @@ cudaError_t fx_launch_policy(const CUtensorMap& map_obs, const CUtensorMap& map_
                              const CUtensorMap& map_h1, const FxPolicyDev& pol, int hidden, int num_envs, int k_pad,
                              const float* noise, unsigned long long seed, unsigned step, void* action, float* logp,
                              float* value, cudaStream_t stream, int env_begin, int env_end, bool tile_sync, bool continuous,
-                             bool greedy) {
+                             bool greedy, bool separate) {
   uint32_t smem = 0;
-  PolicyKernel kernel = continuous ? policy_kernel<true>(hidden, &smem) : policy_kernel<false>(hidden, &smem);
+  PolicyKernel kernel = policy_kernel(hidden, continuous, separate, &smem);
   if (!kernel) return cudaErrorInvalidValue;
   if (env_end < 0) env_end = num_envs;
+  if (separate) tile_sync = false;  // the actor pair's act_flag does not cover the critic pair's observation reads
   cudaLaunchConfig_t lc = {};
-  lc.gridDim = dim3(2 * ((env_end - env_begin + kTileM - 1) / kTileM));  // one CTA pair per 128-env tile
+  // one CTA pair per 128-env tile and network
+  lc.gridDim = dim3((separate ? 4 : 2) * ((env_end - env_begin + kTileM - 1) / kTileM));
   lc.blockDim = dim3(kThreads);
   lc.dynamicSmemBytes = smem;
   lc.stream = stream;

@@ -10,7 +10,9 @@
 #define FX_POLICY_ACTIONS 3
 
 // fp32 parameters the epilogue reads directly (the two weight matrices travel as bf16 through TMA tensor maps);
-// hidden = the policy's width (64, 128, 256 or 512)
+// hidden = the policy's width (64, 128, 256 or 512).  A separate actor and critic (fx_launch_policy(separate)) stacks
+// the two networks, actor first: b1 / b2 [2][hidden], h1 [rows][2 hidden] (the actor's columns first), head_part
+// [rows][2] (one partial sum per network); head_w / head_b keep their layout (rows 0..2 the actor's, row 3 the critic's).
 struct FxPolicyDev {
   const float* b1;      // [hidden]
   const float* b2;      // [hidden]
@@ -29,7 +31,7 @@ struct FxPolicyDev {
 bool fx_policy_width_ok(int hidden);
 // dynamic shared memory of one policy CTA at that width (0 for an unsupported width)
 size_t fx_policy_smem_bytes(int hidden);
-// sets the dynamic shared-memory limit of every width and action mode
+// sets the dynamic shared-memory limit of every width, action mode and network layout
 cudaError_t fx_policy_configure();
 // One policy evaluation for all envs: obs (bf16 [num_envs][k_pad], through map_obs) -> action / log-prob / value.
 // hidden: the width of both layers (fx_policy_width_ok; otherwise cudaErrorInvalidValue, nothing launched).
@@ -38,12 +40,15 @@ cudaError_t fx_policy_configure();
 // noise == nullptr: the in-kernel counter-based generator (seed, step).  greedy: argmax / mean, noise unused.
 // map_w1 / map_w2: boxes of hidden / 2 rows (one CTA's half of the hidden units); map_h1: over FxPolicyDev::h1
 // ([rows][hidden]), box 128 rows.
+// separate: separate actor and critic networks (the stacked layout of FxPolicyDev; map_w1 / map_w2 over 2 hidden rows,
+// map_h1 over 2 hidden columns), two CTA pairs per tile.  It always runs in plain kernel order: tile_sync is ignored,
+// because the actor pair's act_flag would not tell the step kernel that the critic pair has read the observation slot.
 cudaError_t fx_launch_policy(const CUtensorMap& map_obs, const CUtensorMap& map_w1, const CUtensorMap& map_w2,
                              const CUtensorMap& map_h1, const FxPolicyDev& pol, int hidden, int num_envs, int k_pad,
                              const float* noise, unsigned long long seed, unsigned step, void* action, float* logp,
                              float* value, cudaStream_t stream, int env_begin = 0, int env_end = -1,  // env_begin: a multiple of FX_POLICY_TILE_M
                              bool tile_sync = false,  // true: wait for / publish per-tile flags (FxPolicyDev::act_flag ...)
-                             bool continuous = false, bool greedy = false);
+                             bool continuous = false, bool greedy = false, bool separate = false);
 
 // fp32 [rows][cols] (nn.Linear layout) -> bf16 [rows][cols_pad], zero padded
 cudaError_t fx_policy_pack(const float* src, uint16_t* dst, int rows, int cols, int cols_pad, cudaStream_t stream);

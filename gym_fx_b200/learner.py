@@ -30,20 +30,28 @@ from .sharding import allreduce_mean_grads
 class ActorCritic(nn.Module):
     """Shared-body actor-critic in the layout FusedPolicy.set_weights reads (body[0], body[2], pi, v).
     continuous=True (action_space_mode "continuous"): a Gaussian actor, `pi` = Linear(hidden, 1) gives the mean and the
-    parameter `log_std` [1] the state-independent log sigma; forward() then returns (mean [B, 1], value)."""
+    parameter `log_std` [1] the state-independent log sigma; forward() then returns (mean [B, 1], value).
+    separate=True: separate actor and critic networks -- `body` feeds only `pi`, and `critic_body`, built like `body`,
+    feeds `v`, so the value loss does not shape the policy's features (the layout of Stable-Baselines3's and CleanRL's
+    PPO).  The fused loop runs it as two networks (VecFxEnv.make_policy infers `separate` from the module)."""
 
     def __init__(self, obs_dim: int, hidden: int = 256, n_actions: int = 3, continuous: bool = False,
-                 init_log_std: float = 0.0):
+                 init_log_std: float = 0.0, separate: bool = False):
         super().__init__()
         self.body = nn.Sequential(nn.Linear(obs_dim, hidden), nn.Tanh(), nn.Linear(hidden, hidden), nn.Tanh())
         self.pi = nn.Linear(hidden, 1 if continuous else n_actions)
         self.v = nn.Linear(hidden, 1)
         self.continuous = continuous
+        self.separate = separate
         if continuous:
             self.log_std = nn.Parameter(torch.full((1,), float(init_log_std)))
+        if separate:
+            self.critic_body = nn.Sequential(nn.Linear(obs_dim, hidden), nn.Tanh(), nn.Linear(hidden, hidden), nn.Tanh())
 
     def forward(self, obs):
         h = self.body(obs)
+        if self.separate:
+            return self.pi(h), self.v(self.critic_body(obs)).squeeze(-1)
         return self.pi(h), self.v(h).squeeze(-1)
 
 

@@ -494,10 +494,12 @@ class VecFxEnv:
         self.env_params = table
 
     # ------------------------------------------------------------------ closed loop (policy on the device)
-    def make_policy(self, weights=None, hidden: Optional[int] = None) -> "FusedPolicy":
+    def make_policy(self, weights=None, hidden: Optional[int] = None, separate: Optional[bool] = None) -> "FusedPolicy":
         """An actor-critic MLP(obs_dim, hidden, hidden) evaluated by the fused tensor-core kernel (fxenv.h: FxPolicy).
-        hidden: 64, 128, 256 or 512; None takes it from the weights (the rows of w1), or 256 without weights."""
-        return FusedPolicy(self, weights, hidden)
+        hidden: 64, 128, 256 or 512; None takes it from the weights (the rows of w1), or 256 without weights.
+        separate: separate actor and critic networks instead of one shared body; None takes it from the weights (a
+        module with a critic_body, or a dict with w1_v, b1_v, w2_v, b2_v), or False without weights."""
+        return FusedPolicy(self, weights, hidden, separate)
 
     def rollout(self, policy: "FusedPolicy", horizon: int, buffers: Optional[Dict[str, torch.Tensor]] = None,
                 gumbel: Optional[torch.Tensor] = None, seed: int = 0, noise: Optional[torch.Tensor] = None,
@@ -608,11 +610,16 @@ class FusedPolicy:
     shape [1] (dict key "log_std", or the module's .log_std parameter) gives the state-independent log sigma.
     hidden (both layers): 64, 128, 256 or 512.  None takes the width from `weights` (module.body[0].out_features, or the
     rows of weights["w1"]), or HIDDEN = 256 without weights; an explicit width that disagrees with the weights is a
-    ValueError.  The width is fixed for the life of the policy (`self.hidden`)."""
+    ValueError.  The width is fixed for the life of the policy (`self.hidden`).
+    separate (`self.separate`, fixed too): separate actor and critic networks of the same width (fxenv.h:
+    FXENV_POLICY_SEPARATE) -- `body` feeds `pi` and a second trunk `critic_body` feeds `v` (ActorCritic(separate=True));
+    a weight dict adds the critic trunk as w1_v, b1_v, w2_v, b2_v.  None takes it from `weights`, or False without
+    weights; an explicit value that disagrees with the weights is a ValueError."""
 
     HIDDEN = 256
+    CRITIC_KEYS = ("w1_v", "b1_v", "w2_v", "b2_v")   # the critic trunk in a weight dict of a separate policy
 
-    def __init__(self, env: VecFxEnv, weights=None, hidden: Optional[int] = None):
+    def __init__(self, env: VecFxEnv, weights=None, hidden: Optional[int] = None, separate: Optional[bool] = None):
         inferred = None if weights is None else self._width_of(weights)
         if hidden is None:
             hidden = self.HIDDEN if inferred is None else inferred
@@ -620,12 +627,20 @@ class FusedPolicy:
             raise ValueError(f"hidden={hidden} disagrees with the weights, which are {inferred} wide")
         if int(hidden) not in _native.POLICY_WIDTHS:
             raise ValueError(f"policy width must be one of {_native.POLICY_WIDTHS}, got {hidden}")
+        sep = None if weights is None else self._separate_of(weights)
+        if separate is None:
+            separate = bool(sep)
+        elif sep is not None and bool(separate) != sep:
+            raise ValueError(f"separate={separate} disagrees with the weights, which have "
+                             f"{'separate actor and critic trunks' if sep else 'one shared body'}")
         self.env = env
         self.hidden = int(hidden)
+        self.separate = bool(separate)
         self.continuous = env.action_dtype == torch.float32
         self._p = C.c_void_p()
-        rc = env.L.fxenv_policy_create_ex(env._h, self.hidden, C.byref(self._p))
-        _native.check(env.L, env._h, rc, "fxenv_policy_create_ex")
+        flags = _native.POLICY_SEPARATE if self.separate else 0
+        rc = env.L.fxenv_policy_create_ex2(env._h, self.hidden, flags, C.byref(self._p))
+        _native.check(env.L, env._h, rc, "fxenv_policy_create_ex2")
         self._keep = None
         env._policies.append(self)
         if weights is not None:
@@ -638,6 +653,13 @@ class FusedPolicy:
             return int(weights["w1"].shape[0])
         return int(weights.body[0].out_features)
 
+    @classmethod
+    def _separate_of(cls, weights) -> bool:
+        """whether weights hold separate actor and critic trunks (a critic_body, or the w1_v ... keys of a dict)"""
+        if isinstance(weights, dict):
+            return any(k in weights for k in cls.CRITIC_KEYS)
+        return getattr(weights, "critic_body", None) is not None
+
     def sync_timeouts(self) -> int:
         """Polls of the last rollout's tile hand-over that gave up (0 unless something is broken); synchronises."""
         rc = int(self.env.L.fxenv_policy_sync_timeouts(self._p))
@@ -648,7 +670,8 @@ class FusedPolicy:
     def peek(self, what: str, slot: int = 0) -> torch.Tensor:
         """Copy of an internal device buffer of the policy, for tests and debugging (fxenv_policy_peek), ordered on the
         current stream.  what = "obs16": the bf16 observation copy of `slot` (0 or 1) that the kernel reads,
-        [num_envs, k_pad]; "h1": the layer-1 activations of the last evaluation, [num_envs rounded up to 128, hidden]."""
+        [num_envs, k_pad]; "h1": the layer-1 activations of the last evaluation, [num_envs rounded up to 128, hidden]
+        (separate: [..., 2 * hidden], the actor's columns first)."""
         code = {"obs16": _native.PEEK_OBS16, "h1": _native.PEEK_H1}.get(what)
         if code is None:
             raise ValueError(f"what must be 'obs16' or 'h1', got {what!r}")
@@ -656,7 +679,7 @@ class FusedPolicy:
         n = int(L.fxenv_policy_peek(self._p, code, int(slot), None, 0, s))
         if n < 0:
             _native.check(L, self.env._h, n, "fxenv_policy_peek")
-        cols = self.hidden if what == "h1" else (self.env.obs_dim + 63) // 64 * 64
+        cols = self.hidden * (2 if self.separate else 1) if what == "h1" else (self.env.obs_dim + 63) // 64 * 64
         out = torch.empty((n // (2 * cols), cols), dtype=torch.int16, device=self.env.device)
         rc = int(L.fxenv_policy_peek(self._p, code, int(slot), out.data_ptr(), n, s))
         if rc < 0:
@@ -664,10 +687,17 @@ class FusedPolicy:
         return out.view(torch.bfloat16)
 
     def set_weights(self, weights):
+        sep = self._separate_of(weights)
+        if sep != self.separate:
+            raise ValueError("this policy has " + ("separate actor and critic trunks" if self.separate else "one shared body")
+                             + ", the weights " + ("have separate trunks" if sep else "have one shared body"))
         if not isinstance(weights, dict):
             m = weights
             weights = {"w1": m.body[0].weight, "b1": m.body[0].bias, "w2": m.body[2].weight, "b2": m.body[2].bias,
                        "w_pi": m.pi.weight, "b_pi": m.pi.bias, "w_v": m.v.weight, "b_v": m.v.bias}
+            if self.separate:
+                c = m.critic_body
+                weights.update({"w1_v": c[0].weight, "b1_v": c[0].bias, "w2_v": c[2].weight, "b2_v": c[2].bias})
             if self.continuous:
                 if getattr(m, "log_std", None) is None:
                     raise ValueError("continuous action mode needs a log_std parameter of shape [1] on the module")
@@ -676,6 +706,8 @@ class FusedPolicy:
         n_pi = 1 if self.continuous else 3
         shapes = {"w1": (Hd, D), "b1": (Hd,), "w2": (Hd, Hd), "b2": (Hd,), "w_pi": (n_pi, Hd), "b_pi": (n_pi,), "w_v": (Hd,),
                   "b_v": (1,)}
+        if self.separate:
+            shapes.update({"w1_v": (Hd, D), "b1_v": (Hd,), "w2_v": (Hd, Hd), "b2_v": (Hd,)})
         if self.continuous:
             if "log_std" not in weights:
                 raise ValueError("continuous action mode needs weights['log_std'] of shape [1]")
@@ -691,6 +723,9 @@ class FusedPolicy:
             ts[k] = t
         if self.continuous:  # FxPolicyWeights.b_pi in continuous mode: {b_mu, log sigma}
             ts["b_pi"] = torch.cat([ts["b_pi"], ts.pop("log_std")])
+        if self.separate:  # FxPolicyWeights under FXENV_POLICY_SEPARATE: both trunks stacked, the actor's first
+            for k in ("w1", "b1", "w2", "b2"):
+                ts[k] = torch.cat([ts[k], ts.pop(k + "_v")])
         w = _native.FxPolicyWeights(*[ts[k].data_ptr() for k in ("w1", "b1", "w2", "b2", "w_pi", "b_pi", "w_v", "b_v")])
         rc = self.env.L.fxenv_policy_set_weights(self._p, C.byref(w), self.env._stream())
         _native.check(self.env.L, self.env._h, rc, "fxenv_policy_set_weights")

@@ -429,7 +429,9 @@ int fxenv_set_env_params(FxEnv* env, const double* params_host);
 typedef struct FxPolicy FxPolicy;
 
 /* DEVICE pointers to float32 parameters in torch.nn.Linear layout ([out][in] row-major); hidden = the policy's width
- * (fxenv_policy_create_ex). */
+ * (fxenv_policy_create_ex).  A policy created with FXENV_POLICY_SEPARATE (separate actor and critic networks) takes
+ * both trunks stacked, the actor's first: w1 [2][hidden][obs_dim], b1 [2][hidden], w2 [2][hidden][hidden],
+ * b2 [2][hidden]; w_pi / b_pi are the actor's head and w_v / b_v the critic's, as below. */
 typedef struct FxPolicyWeights {
   const float* w1;   /* [hidden][obs_dim] */
   const float* b1;   /* [hidden] */
@@ -462,11 +464,20 @@ typedef struct FxRollout {
 /* fxenv_rollout_ex flags */
 #define FXENV_ROLLOUT_GREEDY 1u   /* evaluation: the most likely action (argmax of the logits / the mean), no sampling */
 
+/* fxenv_policy_create_ex2 flags */
+#define FXENV_POLICY_SEPARATE 1u  /* separate actor and critic networks of the same width instead of one shared body:
+                                   * the actor MLP gives the logits / mean, the critic MLP the value (the default layout
+                                   * of Stable-Baselines3's and CleanRL's PPO).  Each network runs as its own pair of
+                                   * kernel CTAs per 128-env tile.  Its rollouts always hand tiles over in kernel order
+                                   * (FXENV_TILE_SYNC does not apply). */
+
 /* Discrete or continuous, as FxConfig.action_mode.  `hidden` is the width of both hidden layers: 64, 128, 256 or 512
- * (anything else: FXENV_E_INVALID).  A 512-wide policy runs one kernel CTA per SM instead of two.
- * fxenv_policy_create(env, out) is fxenv_policy_create_ex(env, 256, out). */
+ * (anything else: FXENV_E_INVALID).  A 512-wide policy runs one kernel CTA per SM instead of two.  flags:
+ * FXENV_POLICY_* (unknown bits: FXENV_E_INVALID).  fxenv_policy_create(env, out) is fxenv_policy_create_ex(env, 256,
+ * out), and fxenv_policy_create_ex(env, hidden, out) is fxenv_policy_create_ex2(env, hidden, 0, out). */
 int fxenv_policy_create(FxEnv* env, FxPolicy** out);
 int fxenv_policy_create_ex(FxEnv* env, int32_t hidden, FxPolicy** out);
+int fxenv_policy_create_ex2(FxEnv* env, int32_t hidden, uint32_t flags, FxPolicy** out);
 /* Converts / copies the parameters into the policy's own device buffers (stream-ordered; call after every optimiser step). */
 int fxenv_policy_set_weights(FxPolicy* pol, const FxPolicyWeights* weights_dev, void* stream);
 int fxenv_policy_destroy(FxPolicy* pol);
@@ -485,7 +496,8 @@ int fxenv_policy_sync_timeouts(FxPolicy* pol);
 #define FXENV_PEEK_OBS16 0   /* slot 0 | 1: the bf16 observation copy the policy reads, [num_envs][k_pad] (k_pad = obs_dim
                               * rounded up to a multiple of 64, zero pad columns); a rollout's step t reads slot t % 2 */
 #define FXENV_PEEK_H1 1      /* slot 0: the layer-1 activations of the last policy evaluation (after a rollout: the
-                              * bootstrap one), bf16 [num_envs rounded up to a multiple of 128][hidden] */
+                              * bootstrap one), bf16 [num_envs rounded up to a multiple of 128][hidden]; with
+                              * FXENV_POLICY_SEPARATE [...][2 hidden]: the actor's columns, then the critic's */
 /* Test / debugging aid: stream-ordered copy of an internal policy buffer into caller DEVICE memory `dst` of `bytes`
  * bytes.  dst == NULL: returns the byte size needed.  Returns the bytes copied, or <0.  Reads only. */
 int64_t fxenv_policy_peek(FxPolicy* pol, int what, int slot, void* dst, int64_t bytes, void* stream);
