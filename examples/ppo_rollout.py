@@ -15,6 +15,7 @@ minibatch and advantages are normalised with global statistics (gym_fx_b200.lear
     python examples/ppo_rollout.py --hidden 64
     python examples/ppo_rollout.py --separate-critic --updates 5
     python examples/ppo_rollout.py --randomize-costs 1e-4,3e-4
+    python examples/ppo_rollout.py --population 4 --eval-rollouts 2
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 examples/ppo_rollout.py --envs 4096
 
 --action-space continuous trains a Gaussian actor on the Box(-1, 1) action (thresholded to hold / long / short by the
@@ -37,6 +38,11 @@ code.
 --randomize-costs COMM_MAX,SLIP_MAX draws each env's commission and slippage uniformly from [0, COMM_MAX] and [0, SLIP_MAX]
 before every rollout (VecFxEnv.set_env_params: the values change in place, the rollout graph stays), so that the policy
 does not fit one cost model.
+--population M trains M policies side by side on one handle (VecFxEnv.make_policy(members=M)): member m, initialised
+from seed + m (--seed) with its own optimiser, acts for the m-th contiguous slice of the envs (policy.member_envs(m)),
+and one population rollout and one ppo_update_population per update train them all.  The JSON line then also holds
+`members`: per member, the last update's stats and the mean total return of its envs' last finished episodes (and,
+with --eval-rollouts, its greedy evaluation reward).  --envs must be a multiple of 128 x M.
 Prints one JSON line: env-steps/s (decisions) of the rollout phase (policy in the loop) and of the whole train loop, and
 bars/s of the rollout phase as an upper bound (decisions x K: a step that ends an episode runs fewer bars).
 """
@@ -83,6 +89,9 @@ def main():
                     help="the end of an episode window is a truncation (bootstrapped), not a termination")
     ap.add_argument("--randomize-costs", default=None, metavar="COMM_MAX,SLIP_MAX",
                     help="draw each env's commission and slippage uniformly from [0, max] before every rollout")
+    ap.add_argument("--population", type=int, default=1,
+                    help="policies trained side by side, each on its own slice of the envs (1: one policy)")
+    ap.add_argument("--seed", type=int, default=0, help="parameter seed (member m of a population: seed + m)")
     args = ap.parse_args()
     continuous = args.action_space == "continuous"
     cost_max = None
@@ -101,9 +110,12 @@ def main():
         ap.error("--action-repeat must be in 1..256")
     if args.max_episode_steps < 0:
         ap.error("--max-episode-steps must be >= 0")
+    M = args.population
+    if M < 1 or args.envs % (128 * M):
+        ap.error("--population must be >= 1, and --envs a multiple of 128 x --population")
 
     import bench
-    from gym_fx_b200.learner import ActorCritic, ppo_update
+    from gym_fx_b200.learner import ActorCritic, ppo_update, ppo_update_population
     from gym_fx_b200.sharding import check_pair_alignment, shard_starts
     from gym_fx_b200.vec_env import VecFxEnv
 
@@ -162,15 +174,19 @@ def main():
     done_start = env.episode_stats()["episodes_done"].clone()   # the episodes the stagger cut short are not training's
 
     torch.backends.cuda.matmul.allow_tf32 = True
-    torch.manual_seed(0)  # identical replicas on every rank
-    net = ActorCritic(D, hidden=args.hidden, continuous=continuous, separate=args.separate_critic).to(dev)
-    opt = torch.optim.Adam(net.parameters(), lr=args.lr, eps=1e-5)
-    policy = env.make_policy(net)
+    nets = []
+    for m in range(M):
+        torch.manual_seed(args.seed + m)  # identical replicas on every rank
+        nets.append(ActorCritic(D, hidden=args.hidden, continuous=continuous, separate=args.separate_critic).to(dev))
+    opts = [torch.optim.Adam(n.parameters(), lr=args.lr, eps=1e-5) for n in nets]
+    net, opt = nets[0], opts[0]
+    policy = env.make_policy(nets if M > 1 else net)
     buf = None
     prev_done = torch.zeros(N, dtype=torch.uint8, device=dev)
 
     t_roll = t_upd = 0.0
     stats = {}
+    member_stats = [{} for _ in range(M)]   # a population: the last update's stats of each member
     cost_rng = np.random.default_rng(0xC057 + rank) if cost_max else None
     if cost_max:
         desc += f", commission ~ U[0, {cost_max[0]:g}] and slippage ~ U[0, {cost_max[1]:g}] per env and rollout"
@@ -183,9 +199,14 @@ def main():
         buf = env.rollout(policy, H, buffers=buf, seed=1000 * rank + it)
         torch.cuda.synchronize(dev)
         t1 = time.perf_counter()
-        stats = ppo_update(net, opt, buf, prev_done, dist, epochs=args.epochs, minibatches=args.minibatches)
+        if M > 1:
+            member_stats = ppo_update_population(nets, opts, buf, prev_done, dist, epochs=args.epochs,
+                                                 minibatches=args.minibatches)
+            stats = {}
+        else:
+            stats = ppo_update(net, opt, buf, prev_done, dist, epochs=args.epochs, minibatches=args.minibatches)
         prev_done = buf["done"][-1].clone()
-        policy.set_weights(net)                           # bf16 repack of the two hidden layers for the next rollout
+        policy.set_weights(nets if M > 1 else net)        # bf16 repack of the two hidden layers for the next rollout
         torch.cuda.synchronize(dev)
         t2 = time.perf_counter()
         if it > 0:                                        # the first iteration pays one-off set-up costs
@@ -194,12 +215,15 @@ def main():
         d = buf["done"]   # 0 / 1, or the codes 1 = terminated, 2 = truncated with a time limit
         stats.update(mean_reward=float(buf["reward"].mean()), terminated_frac=float((d == 1).float().mean()),
                      truncated_frac=float((d == 2).float().mean()))
+        if M > 1:
+            for m in range(M):
+                member_stats[m]["mean_reward"] = float(buf["reward"][:, policy.member_envs(m)].mean())
 
-    def episode_report(prefix, done_before):
+    def episode_report(prefix, done_before, envs=slice(None)):
         """Episodes finished since `done_before` and the mean total return / max drawdown of each env's last finished one
-        (envs without one are left out), summed / averaged over the ranks."""
-        ep = env.episode_stats()
-        new = (ep["episodes_done"] - done_before).double()
+        (envs without one are left out), summed / averaged over the ranks; `envs`: only these envs (a member's slice)."""
+        ep = {k: v[envs] for k, v in env.episode_stats().items() if k in ("episodes_done", "total_return", "max_drawdown_pct")}
+        new = (ep["episodes_done"] - done_before[envs]).double()
         has = (new > 0).double()
         v = torch.stack([new.sum(), has.sum(), (ep["total_return"] * has).sum(), (ep["max_drawdown_pct"] * has).sum()])
         if dist:
@@ -209,24 +233,35 @@ def main():
                 f"{prefix}_mean_max_drawdown_pct": float(v[3]) / n if v[1] > 0 else None}
 
     holdout = args.holdout_frac > 0.0
+    per_member = range(M) if M > 1 else range(0)   # a population reports each member on its own envs
+    members = [dict(s) for s in member_stats]
     if holdout:   # every env into a fresh episode in the held-out tail; the reset records the training episodes it ends
         env.set_episode_starts(split, T - L, seed=0xE7A10000 + rank)
         env.reset()
         stats.update(episode_report("train", done_start))
         done0 = env.episode_stats()["episodes_done"].clone()
+    for m in per_member:
+        members[m].update(episode_report("train", done_start, policy.member_envs(m)))
     if args.eval_rollouts > 0:   # greedy evaluation of the trained policy (held out: from the fresh episodes)
-        rew_sum = torch.zeros((), dtype=torch.float64, device=dev)
+        rew_sum = torch.zeros(1 + len(per_member), dtype=torch.float64, device=dev)   # all envs, then each member
         for _ in range(args.eval_rollouts):
             buf = env.rollout(policy, H, buffers=buf, deterministic=True)
-            rew_sum += buf["reward"].double().mean()
-        ev = torch.stack([rew_sum / args.eval_rollouts])
+            r = buf["reward"].double()
+            rew_sum[0] += r.mean()
+            for m in per_member:
+                rew_sum[1 + m] += r[:, policy.member_envs(m)].mean()
+        ev = rew_sum / args.eval_rollouts
         if dist:
             dist.all_reduce(ev, op=dist.ReduceOp.SUM)
             ev /= world
         stats["eval_mean_reward"] = float(ev[0])
+        for m in per_member:
+            members[m]["eval_mean_reward"] = float(ev[1 + m])
         if holdout:
             env.reset()          # records the evaluation episodes still running
             stats.update(episode_report("eval", done0))
+            for m in per_member:
+                members[m].update(episode_report("eval", done0, policy.member_envs(m)))
 
     n_it = max(1, args.updates - 1)
     tt = torch.tensor([t_roll, t_upd], dtype=torch.float64, device=dev)
@@ -240,10 +275,11 @@ def main():
             "policy": f"MLP({D},{args.hidden},{args.hidden}) actor-critic, {'separate actor and critic' if args.separate_critic else 'shared body'} "
                       f"({args.action_space} actions), fused wgmma kernel in the rollout, "
                       "torch (tf32) in the update",
-            "hidden": args.hidden, "separate_critic": args.separate_critic, "rollout_env_steps_per_s": steps / max(t_roll, 1e-9), "rollout_us_per_step": t_roll / (H * n_it) * 1e6,
+            "hidden": args.hidden, "separate_critic": args.separate_critic, "population": M, "rollout_env_steps_per_s": steps / max(t_roll, 1e-9), "rollout_us_per_step": t_roll / (H * n_it) * 1e6,
             "action_repeat": K, "repeat_mode": args.repeat_mode, "randomize_costs": list(cost_max) if cost_max else None,
             "rollout_bars_per_s_upper_bound": steps * K / max(t_roll, 1e-9),
-            "train_env_steps_per_s": steps / max(t_roll + t_upd, 1e-9), "update_s": t_upd / n_it, **stats}), flush=True)
+            "train_env_steps_per_s": steps / max(t_roll + t_upd, 1e-9), "update_s": t_upd / n_it, **stats,
+            **({"members": members} if M > 1 else {})}), flush=True)
     env.close()
     if dist:
         dist.barrier()

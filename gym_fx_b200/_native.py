@@ -32,7 +32,8 @@ EXPORTS = [
     "fxenv_policy_create", "fxenv_policy_set_weights", "fxenv_policy_destroy", "fxenv_rollout", "fxenv_policy_sync_timeouts",
     "fxenv_rollout_ex", "fxenv_policy_peek", "fxenv_set_reset_starts", "fxenv_get_episode_info",
     "fxenv_set_bracket_audit", "fxenv_get_bracket_audit", "fxenv_set_action_repeat", "fxenv_policy_create_ex",
-    "fxenv_set_time_limit", "fxenv_set_env_params", "fxenv_policy_create_ex2",
+    "fxenv_set_time_limit", "fxenv_set_env_params", "fxenv_policy_create_ex2", "fxenv_policy_create_ex3",
+    "fxenv_policy_set_member_weights",
 ]
 
 ROLLOUT_GREEDY = 1  # FXENV_ROLLOUT_GREEDY
@@ -141,7 +142,9 @@ def load():
     L.fxenv_policy_create.argtypes = [vp, C.POINTER(vp)]
     L.fxenv_policy_create_ex.argtypes = [vp, C.c_int32, C.POINTER(vp)]
     L.fxenv_policy_create_ex2.argtypes = [vp, C.c_int32, C.c_uint32, C.POINTER(vp)]
+    L.fxenv_policy_create_ex3.argtypes = [vp, C.c_int32, C.c_uint32, C.c_int32, C.POINTER(vp)]
     L.fxenv_policy_set_weights.argtypes = [vp, C.POINTER(FxPolicyWeights), vp]
+    L.fxenv_policy_set_member_weights.argtypes = [vp, C.c_int32, C.POINTER(FxPolicyWeights), vp]
     L.fxenv_policy_destroy.argtypes = [vp]
     L.fxenv_rollout.argtypes = [vp, vp, C.POINTER(FxRollout), vp]
     L.fxenv_rollout_ex.argtypes = [vp, vp, C.POINTER(FxRollout), C.c_uint32, vp]

@@ -828,9 +828,10 @@ struct FxPolicy {
   int hidden = FX_POLICY_HIDDEN;       // width of both hidden layers: 64, 128, 256 or 512 (fxenv_policy_create_ex)
   bool separate = false;               // FXENV_POLICY_SEPARATE: actor and critic trunks, stacked (nets = 2) below
   int nets = 1;                        // trunks: 1 (shared body) or 2 (actor, critic)
-  uint16_t* w1 = nullptr;              // bf16 [nets][hidden][k_pad]
-  uint16_t* w2 = nullptr;              // bf16 [nets][hidden][hidden]
-  float* fparams = nullptr;            // b1[nets][hidden] | b2[nets][hidden] | head_w[4][hidden] | head_b[4]
+  int members = 1;                     // population members (fxenv_policy_create_ex3), each num_envs / members envs
+  uint16_t* w1 = nullptr;              // bf16 [members][nets][hidden][k_pad]
+  uint16_t* w2 = nullptr;              // bf16 [members][nets][hidden][hidden]
+  float* fparams = nullptr;            // b1[members][nets][hidden] | b2[members][nets][hidden] | head_w[members][4][hidden] | head_b[members][4]
   uint16_t* obs16[2] = {nullptr, nullptr};  // bf16 [num_envs][k_pad], double buffered
   uint16_t* h1 = nullptr;              // bf16 [num_envs padded to whole tiles][nets * hidden]: where the halves meet
   float* head_part = nullptr;          // float4 [num_envs padded][nets]: partial head sums of the second CTA of a pair
@@ -843,7 +844,8 @@ struct FxPolicy {
   cudaEvent_t ev_fork = nullptr, ev_join[kGroups - 1] = {};
   CUtensorMap map_obs[2], map_w1, map_w2, map_h1;
   FxPolicyDev dev;
-  bool has_weights = false;
+  std::vector<bool> has_weights;       // [members]: set by fxenv_policy_set_member_weights
+  int missing_weights = 0;             // members without weights: a rollout needs 0
   bool continuous = false;             // FX_ACTION_CONTINUOUS: Gaussian head, float32 actions (fx_policy_kernel<true>)
   struct { cudaGraphExec_t exec = nullptr; FxRollout io; uint32_t flags = 0; uint64_t params_epoch = 0; } cached;
 };
@@ -922,7 +924,7 @@ cudaError_t enqueue_rollout(FxEnv* env, FxPolicy* pol, const FxRollout& io, uint
                            (!last && io.gumbel) ? io.gumbel + (size_t)t * N * noise_per_env : nullptr, io.seed, (unsigned)t,
                            last ? static_cast<void*>(pol->scratch_act) : actions + (size_t)t * N,
                            last ? pol->scratch_logp : io.logp + (size_t)t * N, io.value + (size_t)t * N, sg, (int)e0, (int)e1,
-                           tile_sync, pol->continuous, greedy, pol->separate);
+                           tile_sync, pol->continuous, greedy, pol->separate, pol->tiles / pol->members);
       if (e != cudaSuccess) return e;
       if (last) break;
       const FxTileSync ts = {pol->dev.act_flag, pol->sync + pol->tiles, pol->dev.timeouts, t + 1};
@@ -1000,6 +1002,10 @@ int fxenv_policy_create_ex(FxEnv* env, int32_t hidden, FxPolicy** out) {
 }
 
 int fxenv_policy_create_ex2(FxEnv* env, int32_t hidden, uint32_t flags, FxPolicy** out) {
+  return fxenv_policy_create_ex3(env, hidden, flags, 1, out);
+}
+
+int fxenv_policy_create_ex3(FxEnv* env, int32_t hidden, uint32_t flags, int32_t members, FxPolicy** out) {
   if (!env || !out) return FXENV_E_INVALID;
   *out = nullptr;
   if (flags & ~(uint32_t)FXENV_POLICY_SEPARATE) return fail(env, FXENV_E_INVALID, "unknown policy flags");
@@ -1007,6 +1013,11 @@ int fxenv_policy_create_ex2(FxEnv* env, int32_t hidden, uint32_t flags, FxPolicy
     return fail(env, FXENV_E_INVALID, "unknown action mode");
   if (!fx_policy_width_ok(hidden))
     return fail(env, FXENV_E_INVALID, "policy width must be 64, 128, 256 or 512, got " + std::to_string(hidden));
+  if (members < 1) return fail(env, FXENV_E_INVALID, "policy members must be >= 1, got " + std::to_string(members));
+  if (members > 1 && (int64_t)env->P.cfg.num_envs % ((int64_t)FX_POLICY_TILE_M * members) != 0)
+    return fail(env, FXENV_E_INVALID, "num_envs (" + std::to_string(env->P.cfg.num_envs) + ") must be a multiple of " +
+                                      std::to_string(FX_POLICY_TILE_M) + " x members (" + std::to_string(members) +
+                                      "): each member owns whole 128-env tiles");
   DeviceGuard g(env->device);
   FxPolicy* pol = new (std::nothrow) FxPolicy();
   if (!pol) return fail(env, FXENV_E_NOMEM, "out of host memory");
@@ -1015,11 +1026,14 @@ int fxenv_policy_create_ex2(FxEnv* env, int32_t hidden, uint32_t flags, FxPolicy
   pol->hidden = hidden;
   pol->separate = (flags & FXENV_POLICY_SEPARATE) != 0;
   pol->nets = pol->separate ? 2 : 1;
-  const size_t N = (size_t)env->P.cfg.num_envs, D = (size_t)env->P.obs_dim;
+  pol->members = members;
+  pol->has_weights.assign((size_t)members, false);
+  pol->missing_weights = members;
+  const size_t N = (size_t)env->P.cfg.num_envs, D = (size_t)env->P.obs_dim, M = (size_t)members;
   pol->k_pad = (int)((D + 63) / 64 * 64);
   const size_t KP = (size_t)pol->k_pad, Hd = (size_t)hidden, Hn = (size_t)pol->nets * Hd;  // Hn: stacked trunk rows
-  bool ok = cudaMalloc(&pol->w1, Hn * KP * 2) == cudaSuccess && cudaMalloc(&pol->w2, Hn * Hd * 2) == cudaSuccess &&
-            cudaMalloc(&pol->fparams, (2 * Hn + 4 * Hd + 4) * sizeof(float)) == cudaSuccess &&
+  bool ok = cudaMalloc(&pol->w1, M * Hn * KP * 2) == cudaSuccess && cudaMalloc(&pol->w2, M * Hn * Hd * 2) == cudaSuccess &&
+            cudaMalloc(&pol->fparams, M * (2 * Hn + 4 * Hd + 4) * sizeof(float)) == cudaSuccess &&
             cudaMalloc(&pol->obs16[0], N * KP * 2) == cudaSuccess && cudaMalloc(&pol->obs16[1], N * KP * 2) == cudaSuccess &&
             cudaMalloc(&pol->scratch_act, N * 4) == cudaSuccess && cudaMalloc(&pol->scratch_logp, N * 4) == cudaSuccess;
   const size_t NP = (N + FX_POLICY_TILE_M - 1) / FX_POLICY_TILE_M * FX_POLICY_TILE_M;  // whole 128-env tiles
@@ -1031,16 +1045,17 @@ int fxenv_policy_create_ex2(FxEnv* env, int32_t hidden, uint32_t flags, FxPolicy
   // the K padding of the observation copies is never written by the env kernels: zero it once
   cudaMemset(pol->obs16[0], 0, N * KP * 2);
   cudaMemset(pol->obs16[1], 0, N * KP * 2);
-  pol->dev.b1 = pol->fparams; pol->dev.b2 = pol->fparams + Hn; pol->dev.head_w = pol->fparams + 2 * Hn;
-  pol->dev.head_b = pol->fparams + 2 * Hn + 4 * Hd;
+  pol->dev.b1 = pol->fparams; pol->dev.b2 = pol->fparams + M * Hn; pol->dev.head_w = pol->fparams + 2 * M * Hn;
+  pol->dev.head_b = pol->fparams + 2 * M * Hn + 4 * M * Hd;
   pol->dev.h1 = pol->h1; pol->dev.head_part = reinterpret_cast<float4*>(pol->head_part);
   pol->dev.dbg = env->P.timeline;  // (nullptr unless FXENV_TIMELINE is set; only the timing build looks at it)
   pol->dev.act_flag = pol->sync; pol->dev.done_cnt = pol->sync + pol->tiles; pol->dev.timeouts = pol->sync + 2 * pol->tiles;
   cudaMemset(pol->sync, 0, (2 * (size_t)pol->tiles + 1) * sizeof(int32_t));
   int rc = make_map(env, &pol->map_obs[0], pol->obs16[0], N, KP, FX_POLICY_TILE_M);
   if (!rc) rc = make_map(env, &pol->map_obs[1], pol->obs16[1], N, KP, FX_POLICY_TILE_M);
-  if (!rc) rc = make_map(env, &pol->map_w1, pol->w1, Hn, KP, (uint32_t)Hd / 2);   // a CTA loads its half of the units
-  if (!rc) rc = make_map(env, &pol->map_w2, pol->w2, Hn, Hd, (uint32_t)Hd / 2);
+  // over every member's rows; a CTA loads its half of one network's units
+  if (!rc) rc = make_map(env, &pol->map_w1, pol->w1, M * Hn, KP, (uint32_t)Hd / 2);
+  if (!rc) rc = make_map(env, &pol->map_w2, pol->w2, M * Hn, Hd, (uint32_t)Hd / 2);
   if (!rc) rc = make_map(env, &pol->map_h1, pol->h1, NP, Hn, FX_POLICY_TILE_M);
   if (rc) { fxenv_policy_destroy(pol); return rc; }
   cudaError_t ce = fx_policy_configure();
@@ -1053,19 +1068,29 @@ int fxenv_policy_create_ex2(FxEnv* env, int32_t hidden, uint32_t flags, FxPolicy
 }
 
 int fxenv_policy_set_weights(FxPolicy* pol, const FxPolicyWeights* w, void* stream_) {
+  return fxenv_policy_set_member_weights(pol, 0, w, stream_);
+}
+
+int fxenv_policy_set_member_weights(FxPolicy* pol, int32_t member, const FxPolicyWeights* w, void* stream_) {
   if (!pol || !w) return FXENV_E_INVALID;
   FxEnv* env = pol->env;
+  if (member < 0 || member >= pol->members)
+    return fail(env, FXENV_E_INVALID, "policy member " + std::to_string(member) + " out of range [0, " +
+                                      std::to_string(pol->members) + ")");
   if (!w->w1 || !w->b1 || !w->w2 || !w->b2 || !w->w_pi || !w->b_pi || !w->w_v || !w->b_v) return fail(env, FXENV_E_INVALID, "null weight pointer");
   DeviceGuard g(env->device);
   cudaStream_t s = (cudaStream_t)stream_;
   const int D = env->P.obs_dim, Hd = pol->hidden, Hn = pol->nets * Hd;  // Hn: stacked trunk rows
-  FX_CUDA(env, fx_policy_pack(w->w1, pol->w1, Hn, D, pol->k_pad, s));
-  FX_CUDA(env, fx_policy_pack(w->w2, pol->w2, Hn, Hd, Hd, s));
+  const size_t m = (size_t)member, M = (size_t)pol->members;
+  FX_CUDA(env, fx_policy_pack(w->w1, pol->w1 + m * Hn * pol->k_pad, Hn, D, pol->k_pad, s));
+  FX_CUDA(env, fx_policy_pack(w->w2, pol->w2 + m * Hn * Hd, Hn, Hd, Hd, s));
   float* f = pol->fparams;
-  float* hw = f + 2 * Hn;      // head rows [4][Hd]
-  float* hb = hw + 4 * Hd;     // head bias [4]
-  FX_CUDA(env, cudaMemcpyAsync(f, w->b1, Hn * 4, cudaMemcpyDeviceToDevice, s));
-  FX_CUDA(env, cudaMemcpyAsync(f + Hn, w->b2, Hn * 4, cudaMemcpyDeviceToDevice, s));
+  float* b1 = f + m * Hn;                         // the member's b1 [Hn]
+  float* b2 = f + (M + m) * Hn;                   // its b2 [Hn]
+  float* hw = f + 2 * M * Hn + m * 4 * Hd;        // its head rows [4][Hd]
+  float* hb = f + 2 * M * Hn + 4 * M * Hd + m * 4;  // its head bias [4]
+  FX_CUDA(env, cudaMemcpyAsync(b1, w->b1, Hn * 4, cudaMemcpyDeviceToDevice, s));
+  FX_CUDA(env, cudaMemcpyAsync(b2, w->b2, Hn * 4, cudaMemcpyDeviceToDevice, s));
   if (pol->continuous) {  // head rows {w_mu, 0, 0, w_v}, head bias {b_mu, log sigma, 0, b_v}
     FX_CUDA(env, cudaMemcpyAsync(hw, w->w_pi, Hd * 4, cudaMemcpyDeviceToDevice, s));
     FX_CUDA(env, cudaMemsetAsync(hw + Hd, 0, 2 * Hd * 4, s));
@@ -1078,7 +1103,7 @@ int fxenv_policy_set_weights(FxPolicy* pol, const FxPolicyWeights* w, void* stre
   FX_CUDA(env, cudaMemcpyAsync(hw + 3 * Hd, w->w_v, Hd * 4, cudaMemcpyDeviceToDevice, s));
   FX_CUDA(env, cudaMemcpyAsync(hb + 3, w->b_v, 4, cudaMemcpyDeviceToDevice, s));
   env->launches += 2;
-  pol->has_weights = true;
+  if (!pol->has_weights[m]) { pol->has_weights[m] = true; pol->missing_weights--; }
   return FXENV_OK;
 }
 
@@ -1091,7 +1116,13 @@ int fxenv_rollout_ex(FxEnv* env, FxPolicy* pol, const FxRollout* io, uint32_t fl
   if (rc) return rc;
   if (!pol || !io || pol->env != env) return fail(env, FXENV_E_INVALID, "policy does not belong to this env");
   if (flags & ~(uint32_t)FXENV_ROLLOUT_GREEDY) return fail(env, FXENV_E_INVALID, "unknown rollout flags");
-  if (!pol->has_weights) return fail(env, FXENV_E_STATE, "fxenv_policy_set_weights has not been called");
+  if (pol->missing_weights > 0) {
+    if (pol->members == 1) return fail(env, FXENV_E_STATE, "fxenv_policy_set_weights has not been called");
+    int first = 0;
+    while (pol->has_weights[first]) first++;
+    return fail(env, FXENV_E_STATE, std::to_string(pol->missing_weights) + " of " + std::to_string(pol->members) +
+                                    " policy members have no weights yet (first: member " + std::to_string(first) + ")");
+  }
   if (io->horizon < 1 || io->obs_slots < 2) return fail(env, FXENV_E_INVALID, "horizon must be >= 1 and obs_slots >= 2");
   if (!io->obs || !io->actions || !io->logp || !io->value || !io->reward || !io->done) return fail(env, FXENV_E_INVALID, "null I/O pointer");
   DeviceGuard g(env->device);

@@ -42,6 +42,13 @@
 // and stores action / log-prob, the critic pair stores the value of row 3; head_part holds one float4 per row and
 // network.  No per-tile hand-over: the actor pair's act_flag would not cover the critic pair's reads of the
 // observation slot.
+//
+// Policy population (launch argument tiles_per_member): M members, each a whole actor-critic of the layout above,
+// stacked member-major in every parameter (W1 [M][nets][HID][KP], W2 [M][nets][HID][HID], b1 / b2 [M][nets][HID],
+// head_w [M][4][HID], head_b [M][4]).  Member m owns the 128-env tiles [m tiles_per_member, (m + 1) tiles_per_member);
+// a CTA takes its member from its tile and reads that member's rows and parameters.  h1, head_part, sampling, noise
+// and the tile hand-over are per env row and do not see members.  One member (tiles_per_member >= the tile count) is
+// member 0 everywhere: the kernel above.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -210,13 +217,14 @@ constexpr float kHalfLog2Pi = 0.918938533204672742f;
 // CONT = false: discrete actions (int32, Gumbel-max over 3 logits; noise: float32 [num_envs][3] Gumbel(0,1)).
 // CONT = true:  continuous actions (float32, Gaussian; noise: float32 [num_envs] N(0,1)).
 // SEP = true:   separate actor and critic networks, two CTA pairs per tile (see the top of the file).
+// tiles_per_member: 128-env tiles per population member (see the top of the file).
 template <int HID, bool CONT, bool SEP>
 __global__ void __launch_bounds__(kThreads, Width<HID>::kMinBlocks)
 fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_constant__ CUtensorMap map_w1,
                  const __grid_constant__ CUtensorMap map_w2, const __grid_constant__ CUtensorMap map_h1, const FxPolicyDev pol,
                  const int num_envs, const int k_blocks1, const float* __restrict__ noise, const unsigned long long seed,
                  const unsigned step, void* __restrict__ action_, float* __restrict__ logp, float* __restrict__ value,
-                 const int env_begin, const int tile_sync, const int greedy) {
+                 const int env_begin, const int tile_sync, const int greedy, const int tiles_per_member) {
   using S = Width<HID>;
   constexpr int kHalfN = S::kHalfN, kAcc = S::kAcc;
   constexpr uint32_t kStageBytes = S::kStageBytes, kOffBar = S::kOffBar, kOffHeadW = S::kOffHeadW, kOffBias = S::kOffBias;
@@ -229,9 +237,13 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
   const int rank = blockIdx.x & 1;                         // which half of the hidden units (cluster = CTA pair)
   const int m0 = env_begin + (blockIdx.x >> (SEP ? 2 : 1)) * kTileM;  // a launch covers the envs [env_begin, num_envs)
   const int n0 = rank * kHalfN;
-  // SEP: which network this pair computes; its rows of W1 / W2 / b1 / b2 and its columns of h1 start at net * HID
+  // SEP: which network this pair computes; its columns of h1 start at net * HID
   const int net = SEP ? (int)(blockIdx.x >> 1) & 1 : 0;
-  const int wrow = net * HID + n0;                         // this CTA's first row of W1 / W2, first column of h1
+  constexpr int kNets = SEP ? 2 : 1;
+  const int member = (m0 / kTileM) / tiles_per_member;    // population member of this tile
+  const int trunk = (member * kNets + net) * HID;          // the network's first row of W1 / W2, first entry of b1 / b2
+  const int wrow = trunk + n0;                             // this CTA's first row of W1 / W2
+  const int hcol = net * HID + n0;                         // this CTA's first column of h1
   constexpr int kH1Cols = SEP ? 2 * HID : HID;             // h1 row stride
   constexpr int kParts = SEP ? 2 : 1;                      // head_part float4s per row
   const bool actor = !SEP || net == 0, critic = !SEP || net == 1;
@@ -256,9 +268,9 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   // small fp32 parameters (weights of this launch, not produced by the previous kernel): plain loads
-  for (int i = threadIdx.x; i < 4 * HID; i += kThreads) head_w[i] = pol.head_w[i];
+  for (int i = threadIdx.x; i < 4 * HID; i += kThreads) head_w[i] = pol.head_w[member * 4 * HID + i];
   for (int i = threadIdx.x; i < 2 * HID + 4; i += kThreads)
-    bias[i] = (i < HID) ? pol.b1[net * HID + i] : (i < 2 * HID ? pol.b2[net * HID + i - HID] : pol.head_b[i - 2 * HID]);
+    bias[i] = (i < HID) ? pol.b1[trunk + i] : (i < 2 * HID ? pol.b2[trunk + i - HID] : pol.head_b[member * 4 + i - 2 * HID]);
   __syncthreads();
   asm volatile("griddepcontrol.launch_dependents;");  // the env step that consumes our actions may get scheduled early
   const int kb2 = HID / kBlockK;             // k-blocks of layer 2 (1, 2, 4, 8)
@@ -329,7 +341,7 @@ fx_policy_kernel(const __grid_constant__ CUtensorMap map_obs, const __grid_const
       if (lane == 0) mbar_arrive(&bar->empty[s]);
     }
     const float* b1 = bias + n0;
-    uint32_t* h_lo = reinterpret_cast<uint32_t*>(pol.h1 + (size_t)(m0 + r_lo) * kH1Cols + wrow + c_lane);
+    uint32_t* h_lo = reinterpret_cast<uint32_t*>(pol.h1 + (size_t)(m0 + r_lo) * kH1Cols + hcol + c_lane);
     uint32_t* h_hi = h_lo + 8 * kH1Cols / 2;
 #pragma unroll
     for (int j = 0; j < kAcc / 4; j++) {
@@ -514,10 +526,10 @@ cudaError_t fx_launch_policy(const CUtensorMap& map_obs, const CUtensorMap& map_
                              const CUtensorMap& map_h1, const FxPolicyDev& pol, int hidden, int num_envs, int k_pad,
                              const float* noise, unsigned long long seed, unsigned step, void* action, float* logp,
                              float* value, cudaStream_t stream, int env_begin, int env_end, bool tile_sync, bool continuous,
-                             bool greedy, bool separate) {
+                             bool greedy, bool separate, int tiles_per_member) {
   uint32_t smem = 0;
   PolicyKernel kernel = policy_kernel(hidden, continuous, separate, &smem);
-  if (!kernel) return cudaErrorInvalidValue;
+  if (!kernel || tiles_per_member < 1) return cudaErrorInvalidValue;
   if (env_end < 0) env_end = num_envs;
   if (separate) tile_sync = false;  // the actor pair's act_flag does not cover the critic pair's observation reads
   cudaLaunchConfig_t lc = {};
@@ -535,5 +547,5 @@ cudaError_t fx_launch_policy(const CUtensorMap& map_obs, const CUtensorMap& map_
   lc.numAttrs = 2;
   return cudaLaunchKernelEx(&lc, kernel, map_obs, map_w1, map_w2, map_h1,
                             pol, env_end, k_pad / kBlockK, noise, seed, step, action, logp, value, env_begin,
-                            (tile_sync && pol.act_flag) ? 1 : 0, greedy ? 1 : 0);
+                            (tile_sync && pol.act_flag) ? 1 : 0, greedy ? 1 : 0, tiles_per_member);
 }

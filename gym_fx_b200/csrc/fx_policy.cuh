@@ -13,6 +13,8 @@
 // hidden = the policy's width (64, 128, 256 or 512).  A separate actor and critic (fx_launch_policy(separate)) stacks
 // the two networks, actor first: b1 / b2 [2][hidden], h1 [rows][2 hidden] (the actor's columns first), head_part
 // [rows][2] (one partial sum per network); head_w / head_b keep their layout (rows 0..2 the actor's, row 3 the critic's).
+// A population of M members (fx_launch_policy(tiles_per_member)) stacks whole members, member-major: b1 / b2
+// [M][nets][hidden], head_w [M][4][hidden], head_b [M][4]; h1 and head_part are per env row and keep their layout.
 struct FxPolicyDev {
   const float* b1;      // [hidden]
   const float* b2;      // [hidden]
@@ -43,12 +45,15 @@ cudaError_t fx_policy_configure();
 // separate: separate actor and critic networks (the stacked layout of FxPolicyDev; map_w1 / map_w2 over 2 hidden rows,
 // map_h1 over 2 hidden columns), two CTA pairs per tile.  It always runs in plain kernel order: tile_sync is ignored,
 // because the actor pair's act_flag would not tell the step kernel that the critic pair has read the observation slot.
+// tiles_per_member (>= 1, else cudaErrorInvalidValue): the 128-env tiles of each population member; the tile of envs
+// [128 t, 128 t + 128) runs member t / tiles_per_member (the stacked layout of FxPolicyDev; map_w1 / map_w2 over all
+// members' rows).  A value of at least the tile count is a single policy, member 0.
 cudaError_t fx_launch_policy(const CUtensorMap& map_obs, const CUtensorMap& map_w1, const CUtensorMap& map_w2,
                              const CUtensorMap& map_h1, const FxPolicyDev& pol, int hidden, int num_envs, int k_pad,
                              const float* noise, unsigned long long seed, unsigned step, void* action, float* logp,
-                             float* value, cudaStream_t stream, int env_begin = 0, int env_end = -1,  // env_begin: a multiple of FX_POLICY_TILE_M
-                             bool tile_sync = false,  // true: wait for / publish per-tile flags (FxPolicyDev::act_flag ...)
-                             bool continuous = false, bool greedy = false, bool separate = false);
+                             float* value, cudaStream_t stream, int env_begin, int env_end,  // env_begin: a multiple of FX_POLICY_TILE_M; env_end < 0: num_envs
+                             bool tile_sync,  // true: wait for / publish per-tile flags (FxPolicyDev::act_flag ...)
+                             bool continuous, bool greedy, bool separate, int tiles_per_member);
 
 // fp32 [rows][cols] (nn.Linear layout) -> bf16 [rows][cols_pad], zero padded
 cudaError_t fx_policy_pack(const float* src, uint16_t* dst, int rows, int cols, int cols_pad, cudaStream_t stream);

@@ -18,7 +18,7 @@ Limits in Reinforcement Learning", 2018).
 from __future__ import annotations
 
 import math
-from typing import Dict, Optional
+from typing import Dict, List, Optional
 
 import torch
 import torch.nn as nn
@@ -160,3 +160,20 @@ def ppo_update(net: ActorCritic, opt, buf: Dict[str, torch.Tensor], prev_done: t
             opt.step()
             stats = {"loss": loss.detach(), "entropy": ent.detach(), "value_loss": vloss.detach()}
     return {k: float(v) for k, v in stats.items()} | {"valid_frac": float(valid.mean())}
+
+
+def ppo_update_population(nets, opts, buf: Dict[str, torch.Tensor], prev_done: torch.Tensor, dist=None,
+                          **kw) -> List[Dict[str, float]]:
+    """One PPO update of every member of a policy population (VecFxEnv.make_policy(members=M)) from one rollout buffer:
+    ppo_update(nets[m], opts[m], ...) on member m's envs, the contiguous slice [m N / M, (m + 1) N / M) of every
+    buffer's env axis and of prev_done, members in order.  Each member's advantages are normalised over its own envs
+    on all ranks.  kw: ppo_update's keyword arguments.  Returns one stats dict per member."""
+    M = len(nets)
+    if M < 1 or len(opts) != M:
+        raise ValueError(f"{M} networks and {len(opts)} optimisers: one optimiser per member")
+    N = int(buf["reward"].shape[1])
+    if N % M:
+        raise ValueError(f"{N} envs do not split into {M} equal member slices")
+    n = N // M
+    return [ppo_update(nets[m], opts[m], {k: v[:, m * n:(m + 1) * n] for k, v in buf.items()},
+                       prev_done[m * n:(m + 1) * n], dist, **kw) for m in range(M)]

@@ -494,12 +494,16 @@ class VecFxEnv:
         self.env_params = table
 
     # ------------------------------------------------------------------ closed loop (policy on the device)
-    def make_policy(self, weights=None, hidden: Optional[int] = None, separate: Optional[bool] = None) -> "FusedPolicy":
+    def make_policy(self, weights=None, hidden: Optional[int] = None, separate: Optional[bool] = None,
+                    members: Optional[int] = None) -> "FusedPolicy":
         """An actor-critic MLP(obs_dim, hidden, hidden) evaluated by the fused tensor-core kernel (fxenv.h: FxPolicy).
         hidden: 64, 128, 256 or 512; None takes it from the weights (the rows of w1), or 256 without weights.
         separate: separate actor and critic networks instead of one shared body; None takes it from the weights (a
-        module with a critic_body, or a dict with w1_v, b1_v, w2_v, b2_v), or False without weights."""
-        return FusedPolicy(self, weights, hidden, separate)
+        module with a critic_body, or a dict with w1_v, b1_v, w2_v, b2_v), or False without weights.
+        members: a population of that many independent networks of one width and layout, member m acting for the
+        envs `policy.member_envs(m)` (num_envs must then be a multiple of 128 * members); `weights` is then a list or
+        tuple with one module or dict per member.  None takes len(weights) for a list or tuple, else 1."""
+        return FusedPolicy(self, weights, hidden, separate, members)
 
     def rollout(self, policy: "FusedPolicy", horizon: int, buffers: Optional[Dict[str, torch.Tensor]] = None,
                 gumbel: Optional[torch.Tensor] = None, seed: int = 0, noise: Optional[torch.Tensor] = None,
@@ -614,20 +618,39 @@ class FusedPolicy:
     separate (`self.separate`, fixed too): separate actor and critic networks of the same width (fxenv.h:
     FXENV_POLICY_SEPARATE) -- `body` feeds `pi` and a second trunk `critic_body` feeds `v` (ActorCritic(separate=True));
     a weight dict adds the critic trunk as w1_v, b1_v, w2_v, b2_v.  None takes it from `weights`, or False without
-    weights; an explicit value that disagrees with the weights is a ValueError."""
+    weights; an explicit value that disagrees with the weights is a ValueError.
+    members (`self.members`, fixed too): a population of independent networks of that one width and layout (fxenv.h:
+    fxenv_policy_create_ex3); member m acts for the envs `member_envs(m)` and gives there exactly what a single policy
+    with its weights gives.  Weights come as a list or tuple of one module or dict per member (`set_weights`), or one
+    member at a time (`set_member_weights`); members whose weights disagree on the width or layout are a ValueError."""
 
     HIDDEN = 256
     CRITIC_KEYS = ("w1_v", "b1_v", "w2_v", "b2_v")   # the critic trunk in a weight dict of a separate policy
 
-    def __init__(self, env: VecFxEnv, weights=None, hidden: Optional[int] = None, separate: Optional[bool] = None):
-        inferred = None if weights is None else self._width_of(weights)
+    def __init__(self, env: VecFxEnv, weights=None, hidden: Optional[int] = None, separate: Optional[bool] = None,
+                 members: Optional[int] = None):
+        listed = isinstance(weights, (list, tuple))
+        if members is None:
+            members = len(weights) if listed else 1
+        if isinstance(members, bool) or not isinstance(members, (int, np.integer)) or members < 1:
+            raise ValueError(f"members must be an integer >= 1, got {members!r}")
+        members = int(members)
+        if listed and len(weights) != members:
+            raise ValueError(f"{len(weights)} weight sets for a population of {members} members")
+        if weights is not None and not listed and members != 1:
+            raise ValueError(f"a population of {members} members takes a list of {members} weight sets")
+        if members > 1 and env.num_envs % (128 * members):
+            raise ValueError(f"num_envs ({env.num_envs}) must be a multiple of 128 x members ({members}): each member "
+                             "owns whole 128-env tiles")
+        each = None if weights is None else (list(weights) if listed else [weights])
+        inferred = None if each is None else self._common(each, self._width_of, "width")
         if hidden is None:
             hidden = self.HIDDEN if inferred is None else inferred
         elif inferred is not None and int(hidden) != inferred:
             raise ValueError(f"hidden={hidden} disagrees with the weights, which are {inferred} wide")
         if int(hidden) not in _native.POLICY_WIDTHS:
             raise ValueError(f"policy width must be one of {_native.POLICY_WIDTHS}, got {hidden}")
-        sep = None if weights is None else self._separate_of(weights)
+        sep = None if each is None else self._common(each, self._separate_of, "layout (shared body or separate trunks)")
         if separate is None:
             separate = bool(sep)
         elif sep is not None and bool(separate) != sep:
@@ -636,15 +659,25 @@ class FusedPolicy:
         self.env = env
         self.hidden = int(hidden)
         self.separate = bool(separate)
+        self.members = members
         self.continuous = env.action_dtype == torch.float32
         self._p = C.c_void_p()
         flags = _native.POLICY_SEPARATE if self.separate else 0
-        rc = env.L.fxenv_policy_create_ex2(env._h, self.hidden, flags, C.byref(self._p))
-        _native.check(env.L, env._h, rc, "fxenv_policy_create_ex2")
+        rc = env.L.fxenv_policy_create_ex3(env._h, self.hidden, flags, self.members, C.byref(self._p))
+        _native.check(env.L, env._h, rc, "fxenv_policy_create_ex3")
         self._keep = None
+        self._w: Dict[int, Dict[str, torch.Tensor]] = {}
         env._policies.append(self)
         if weights is not None:
             self.set_weights(weights)
+
+    @staticmethod
+    def _common(each, of, what):
+        """the value `of` gives for every member's weights; members that disagree are a ValueError"""
+        vals = [of(w) for w in each]
+        if any(v != vals[0] for v in vals):
+            raise ValueError(f"the members' weights disagree on the {what}: {vals}")
+        return vals[0]
 
     @staticmethod
     def _width_of(weights) -> int:
@@ -686,7 +719,39 @@ class FusedPolicy:
             _native.check(L, self.env._h, rc, "fxenv_policy_peek")
         return out.view(torch.bfloat16)
 
+    def member_envs(self, m: int) -> slice:
+        """The envs member m acts for: [m N / members, (m + 1) N / members) of the handle's N envs."""
+        self._check_member(m)
+        n = self.env.num_envs // self.members
+        return slice(int(m) * n, (int(m) + 1) * n)
+
+    def _check_member(self, m):
+        if isinstance(m, bool) or not isinstance(m, (int, np.integer)) or not 0 <= m < self.members:
+            raise ValueError(f"member must be an integer in [0, {self.members}), got {m!r}")
+
     def set_weights(self, weights):
+        """New parameters for every member: one module or weight dict, or for a population a list or tuple of one per
+        member.  Every set is checked before any is written."""
+        each = list(weights) if isinstance(weights, (list, tuple)) else [weights]
+        if len(each) != self.members:
+            raise ValueError(f"{len(each)} weight sets for a policy of {self.members} member(s)")
+        for m, ts in enumerate([self._tensors(w) for w in each]):
+            self._upload(m, ts)
+
+    def set_member_weights(self, m: int, weights):
+        """New parameters for member m only (a module or weight dict of this policy's width and layout); the other
+        members keep theirs, and the cached rollout graph stays."""
+        self._check_member(m)
+        self._upload(int(m), self._tensors(weights))
+
+    def _upload(self, m: int, ts: Dict[str, torch.Tensor]):
+        w = _native.FxPolicyWeights(*[ts[k].data_ptr() for k in ("w1", "b1", "w2", "b2", "w_pi", "b_pi", "w_v", "b_v")])
+        rc = self.env.L.fxenv_policy_set_member_weights(self._p, m, C.byref(w), self.env._stream())
+        _native.check(self.env.L, self.env._h, rc, "fxenv_policy_set_member_weights")
+        self._w[m] = ts  # keep the sources alive until the stream-ordered copies have run
+
+    def _tensors(self, weights) -> Dict[str, torch.Tensor]:
+        """float32 device tensors in the FxPolicyWeights layout of this policy, checked against its width and layout"""
         sep = self._separate_of(weights)
         if sep != self.separate:
             raise ValueError("this policy has " + ("separate actor and critic trunks" if self.separate else "one shared body")
@@ -726,10 +791,7 @@ class FusedPolicy:
         if self.separate:  # FxPolicyWeights under FXENV_POLICY_SEPARATE: both trunks stacked, the actor's first
             for k in ("w1", "b1", "w2", "b2"):
                 ts[k] = torch.cat([ts[k], ts.pop(k + "_v")])
-        w = _native.FxPolicyWeights(*[ts[k].data_ptr() for k in ("w1", "b1", "w2", "b2", "w_pi", "b_pi", "w_v", "b_v")])
-        rc = self.env.L.fxenv_policy_set_weights(self._p, C.byref(w), self.env._stream())
-        _native.check(self.env.L, self.env._h, rc, "fxenv_policy_set_weights")
-        self._w = ts  # keep the sources alive until the stream-ordered copies have run
+        return ts
 
     def close(self):
         if self._p:

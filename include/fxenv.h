@@ -478,8 +478,21 @@ typedef struct FxRollout {
 int fxenv_policy_create(FxEnv* env, FxPolicy** out);
 int fxenv_policy_create_ex(FxEnv* env, int32_t hidden, FxPolicy** out);
 int fxenv_policy_create_ex2(FxEnv* env, int32_t hidden, uint32_t flags, FxPolicy** out);
-/* Converts / copies the parameters into the policy's own device buffers (stream-ordered; call after every optimiser step). */
+/* Policy population: `members` (>= 1) independent actor-critic networks of one width and layout (flags), each on its
+ * own contiguous slice of the envs: member m acts for envs [m N / members, (m + 1) N / members), N = num_envs.  On its
+ * slice a member gives bit for bit what a single policy with its weights gives there, from the same state and noise
+ * (caller noise, the in-kernel generator and greedy mode alike).  members > 1 needs N to be a multiple of
+ * 128 x members, so that no 128-env kernel tile mixes members; members < 1 or an N that does not divide:
+ * FXENV_E_INVALID.  fxenv_policy_create_ex2(env, hidden, flags, out) is fxenv_policy_create_ex3(env, hidden, flags,
+ * 1, out).  A rollout runs every member in the same kernels as one policy. */
+int fxenv_policy_create_ex3(FxEnv* env, int32_t hidden, uint32_t flags, int32_t members, FxPolicy** out);
+/* Converts / copies the parameters into the policy's own device buffers (stream-ordered; call after every optimiser
+ * step).  fxenv_policy_set_weights(pol, w, s) is fxenv_policy_set_member_weights(pol, 0, w, s). */
 int fxenv_policy_set_weights(FxPolicy* pol, const FxPolicyWeights* weights_dev, void* stream);
+/* The same for one member of a population (FxPolicyWeights as for a single policy of the population's width and
+ * layout); member outside [0, members): FXENV_E_INVALID.  A rollout needs weights for every member (FXENV_E_STATE
+ * until then).  Updating one member leaves the others' parameters and the cached rollout graph as they are. */
+int fxenv_policy_set_member_weights(FxPolicy* pol, int32_t member, const FxPolicyWeights* weights_dev, void* stream);
 int fxenv_policy_destroy(FxPolicy* pol);
 /* `horizon` closed-loop steps starting from the env's current state; everything is enqueued on `stream`
  * (2 * horizon + 2 kernels; the launch sequence is cached as a CUDA graph per buffer set and flags).
