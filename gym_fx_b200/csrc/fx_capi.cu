@@ -8,6 +8,7 @@
 
 #include <new>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "fx_kernels.cuh"
@@ -17,16 +18,34 @@ namespace {
 
 thread_local std::string g_create_error;
 
-struct SlabPlan {
-  size_t bytes = 0;
-  size_t add(size_t nbytes) {
-    const size_t off = bytes;
-    bytes += (nbytes + 255) & ~(size_t)255;
-    return off;
-  }
+}  // namespace
+
+// Instantiated CUDA graphs of launch sequences (launch_cached), one per slot, each stored with the key it was captured
+// for and the handle's params_epoch at the capture: the graphs capture the kernel parameters (FxEnv::P) by value, so a
+// slot of an older epoch is captured again.
+template <typename Key, int Slots>
+struct GraphCache {
+  static_assert(std::has_unique_object_representations_v<Key>, "keys are compared bytewise: no padding");
+  struct Slot {
+    cudaGraphExec_t exec = nullptr;
+    Key key;
+    uint64_t epoch = 0, used = 0;
+  } slot[Slots];
+  uint64_t clock = 0;  // `used` of the last launched slot: the least recently used slot is replaced
+  ~GraphCache() { for (auto& s : slot) if (s.exec) cudaGraphExecDestroy(s.exec); }
 };
 
-}  // namespace
+struct StepManyKey {
+  const void* actions;
+  float *obs, *reward;
+  uint8_t* term;
+  int32_t steps, slots;
+};
+
+struct RolloutKey {
+  FxRollout io;
+  uint64_t flags;  // FXENV_ROLLOUT_*, 64 bits wide so that the key has no padding
+};
 
 struct FxEnv {
   FxKernelParams P;
@@ -54,28 +73,17 @@ struct FxEnv {
   float* h_obs = nullptr;
   float* h_reward = nullptr;
   uint8_t* h_term = nullptr;
-  // fxenv_step_many graph cache (one entry: the last pointer set)
   // fxenv_step_many, graph engine: the two most recent launch sequences, keyed by the pointer set and sizes
-  struct CachedGraph {
-    cudaGraphExec_t exec = nullptr;
-    const void* actions = nullptr;
-    float* obs = nullptr;
-    float* reward = nullptr;
-    uint8_t* term = nullptr;
-    int steps = 0, slots = 0;
-    uint64_t used = 0;
-  } graphs[2];
-  uint64_t graph_clock = 0;
-  // bumped whenever a setting in the kernel parameters changes (the bracket audit, the action repeat, the time limit): a cached rollout
-  // graph captured the old P by value (FxPolicy::cached)
+  GraphCache<StepManyKey, 2> step_graphs;
+  // bumped by params_changing whenever a launch parameter in P changes: every cached graph captured the old P by value
   uint64_t params_epoch = 0;
-  bool trunc_configured = false;   // fx_configure_trunc_kernels has run (fxenv_set_time_limit)
+  // the deferred kernel bits (FX_V_TRUNC, FX_V_PARAMS) ever turned on: the kernel halves they cover are configured
+  unsigned deferred = 0u;
   // per-env parameters (fxenv_set_env_params): the host copy of the table while it is on (the LEAN choice is made on its
   // values).  The device table lives behind the sequence words in the allocation of P.seq, at params_off (0: not yet
   // allocated); P.env_params_off is params_off while the table is on and 0 while it is off.
   std::vector<double> params_host;
   uint32_t params_off = 0;
-  bool params_configured = false;  // fx_configure_params_kernels has run (the truncation half too once trunc_configured)
 };
 
 namespace {
@@ -143,19 +151,97 @@ int require_ready(FxEnv* env, bool need_reset) {
   return FXENV_OK;
 }
 
-void drop_graph(FxEnv* env) {
-  for (auto& g : env->graphs)
-    if (g.exec) { cudaGraphExecDestroy(g.exec); g.exec = nullptr; }
-}
-
-// A launch parameter in env->P is about to change: wait until no launch may still run with the old one (no cached
-// graph is destroyed while a launch of it may be running), drop the cached step-many graphs, which captured the old P,
-// and bump the epoch, so that each policy re-captures its rollout graph on its next use
+// A launch parameter in env->P is about to change: wait until no launch may still run with the old one, and bump the
+// epoch, so that every cached graph (step-many and rollout), which captured the old P, is captured again on its next use
 int params_changing(FxEnv* env) {
   FX_CUDA(env, cudaDeviceSynchronize());
-  drop_graph(env);
   env->params_epoch++;
   return FXENV_OK;
+}
+
+// Runs the launch sequence enqueue(stream) through `cache`: replays the graph captured for `key` at the current
+// params_epoch, or first captures and instantiates one in the least recently used slot.  Inside someone else's capture
+// (e.g. a torch CUDA graph), on the legacy stream, or with `direct`, the sequence is launched as it is.
+template <typename Key, int Slots, typename Enqueue>
+int launch_cached(FxEnv* env, GraphCache<Key, Slots>& cache, const Key& key, bool direct, cudaStream_t stream,
+                  const Enqueue& enqueue, const char* what) {
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  if (stream != nullptr) cudaStreamIsCapturing(stream, &cs);
+  if (direct || cs != cudaStreamCaptureStatusNone || stream == nullptr) {
+    FX_CUDA(env, enqueue(stream));
+    return FXENV_OK;
+  }
+  typename GraphCache<Key, Slots>::Slot* s = nullptr;
+  for (auto& c : cache.slot)
+    if (c.exec && c.epoch == env->params_epoch && memcmp(&c.key, &key, sizeof key) == 0) s = &c;
+  if (!s) {
+    s = &cache.slot[0];
+    for (auto& c : cache.slot) if (c.used < s->used) s = &c;
+    if (s->exec) { cudaGraphExecDestroy(s->exec); s->exec = nullptr; }
+    cudaGraph_t graph = nullptr;
+    FX_CUDA(env, cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
+    cudaError_t e = enqueue(stream);
+    const cudaError_t e2 = cudaStreamEndCapture(stream, &graph);
+    if (e != cudaSuccess) { if (graph) cudaGraphDestroy(graph); return cuda_fail(env, e, what); }
+    if (e2 != cudaSuccess) return cuda_fail(env, e2, "cudaStreamEndCapture");
+    e = cudaGraphInstantiate(&s->exec, graph, 0);
+    cudaGraphDestroy(graph);
+    if (e != cudaSuccess) { s->exec = nullptr; return cuda_fail(env, e, "cudaGraphInstantiate"); }
+    s->key = key;
+    s->epoch = env->params_epoch;
+  }
+  s->used = ++cache.clock;
+  FX_CUDA(env, cudaGraphLaunch(s->exec, stream));
+  return FXENV_OK;
+}
+
+// A setter turns the deferred kernel bit `bit` (FX_V_TRUNC or FX_V_PARAMS) on: configures every kernel half whose bits
+// are now all on for the first time -- their attributes, and the persistent grid's minimum over them (every launch
+// reads the grid and advances the ticket words by its own warp count)
+int use_deferred(FxEnv* env, unsigned bit) {
+  const unsigned on = env->deferred | bit;
+  for (const unsigned half : std::initializer_list<unsigned>{FX_V_TRUNC, FX_V_PARAMS, FX_V_TRUNC | FX_V_PARAMS})
+    if ((half & ~on) == 0u && (half & ~env->deferred) != 0u) FX_CUDA(env, fx_configure_half(env->P, half));
+  env->deferred = on;
+  return FXENV_OK;
+}
+
+// The per-env state slab, described once: every column in slab order with its element count, each column's bytes
+// rounded up to 256.  Returns the slab's size; given the allocation (`base`) it also points the columns into it.  The
+// order and the rounding are the layout of a snapshot blob (fxenv_get_state).
+size_t slab_layout(FxKernelParams& P, unsigned char* base) {
+  const size_t N = (size_t)P.cfg.num_envs, capP = (size_t)P.cap + FXO_SLACK;
+  const size_t ring = (P.cfg.reward == FX_REWARD_SHARPE) ? (size_t)P.cfg.sharpe_window : 1;
+  size_t off = 0;
+  const auto col = [&](auto*& p, size_t n) {
+    if (base) p = reinterpret_cast<std::remove_reference_t<decltype(p)>>(base + off);
+    off += (n * sizeof(*p) + 255) & ~(size_t)255;
+  };
+  FxDeviceState& st = P.st;
+  for (double** p : {&st.cash, &st.psize, &st.pprice, &st.equity, &st.prev_equity, &st.price, &st.commission_paid,
+                     &st.dd_peak, &st.sub_need})
+    col(*p, N);
+  col(st.start, N);
+  col(st.nbar, N * 6);
+  col(st.rstats, N * FX_RS_N);
+  for (int32_t** p : {&st.t, &st.total_bars, &st.position, &st.bar_index, &st.trades, &st.n_orders, &st.sh_len,
+                      &st.sh_head, &st.sh_last_step, &st.dd_last_step, &st.n_acc})
+    col(*p, N);
+  col(st.flags, N);
+  col(st.sh_ring, N * ring);
+  col(st.welford, N * FXENV_MAX_FEATURES * 2);
+  col(st.o_meta, N * capP);
+  col(st.o_p0, N * capP);
+  col(st.o_p1, N * capP);
+  col(st.o_sz, N * capP);
+  col(st.ep_lo, N);
+  col(st.ep_span, N);
+  col(st.ep_seed, 1);
+  col(st.ep_begun, N);
+  col(st.ep_done, N);
+  col(st.ep_last, N * FXENV_EPISODE_STATS);
+  col(P.ep_steps, N);
+  return off;
 }
 
 // Whether the handle runs the LEAN kernels (fx_config_is_lean): decided once every candle table is loaded, on the costs
@@ -203,6 +289,12 @@ int fxenv_create(const FxConfig* cfg, FxEnv** out) {
   env->P.cfg = *cfg;
   FxConfig& c = env->P.cfg;
   if (cudaGetDevice(&env->device) != cudaSuccess) { delete env; return fail(nullptr, FXENV_E_CUDA, "cudaGetDevice failed"); }
+  // FX_CUDA for what follows: frees what was allocated so far, and the message goes to fxenv_last_error(NULL)
+#define FX_CREATE(call)                                                                  \
+  do {                                                                                   \
+    cudaError_t e__ = (call);                                                            \
+    if (e__ != cudaSuccess) { fxenv_destroy(env); return cuda_fail(nullptr, e__, #call); } \
+  } while (0)
   int cap = c.order_capacity == 0 ? 128 : c.order_capacity;
   cap = (cap + 31) & ~31;
   c.order_capacity = cap;
@@ -213,8 +305,8 @@ int fxenv_create(const FxConfig* cfg, FxEnv** out) {
   if (const char* dv = getenv("FXENV_DEBUG")) env->P.debug = atoi(dv);  // timing experiments only
   if (const char* tv = getenv("FXENV_TIMING")) {
     if (atoi(tv)) {
-      cudaMalloc(&env->P.timing, (size_t)c.num_envs * 2 * FX_NSTAMP * sizeof(long long));
-      cudaMemset(env->P.timing, 0, (size_t)c.num_envs * 2 * FX_NSTAMP * sizeof(long long));
+      FX_CREATE(cudaMalloc(&env->P.timing, (size_t)c.num_envs * 2 * FX_NSTAMP * sizeof(long long)));
+      FX_CREATE(cudaMemset(env->P.timing, 0, (size_t)c.num_envs * 2 * FX_NSTAMP * sizeof(long long)));
     }
   }
   env->P.fast_features = 0;
@@ -226,8 +318,8 @@ int fxenv_create(const FxConfig* cfg, FxEnv** out) {
     if (atoi(tl) > 0) {
       env->timeline_steps = atoi(tl);
       const size_t nb = (size_t)env->timeline_steps * c.num_envs * 2 * sizeof(long long);
-      cudaMalloc(&env->P.timeline, nb);
-      cudaMemset(env->P.timeline, 0, nb);
+      FX_CREATE(cudaMalloc(&env->P.timeline, nb));
+      FX_CREATE(cudaMemset(env->P.timeline, 0, nb));
     }
   }
   if (const char* fe = getenv("FXENV_ENGINE")) env->force_engine = (fe[0] == 'p') ? 1 : (fe[0] == 'g' ? 0 : -1);
@@ -240,58 +332,14 @@ int fxenv_create(const FxConfig* cfg, FxEnv** out) {
     if (atoi(rb) > 0 && atoi(rb) < env->P.resident_blocks) env->P.resident_blocks = atoi(rb);
   if (ce != cudaSuccess) { fxenv_destroy(env); return cuda_fail(nullptr, ce, "window_size * n_cols too large for shared memory"); }
   // one slab for the whole per-env state (snapshot == one memcpy)
+  env->slab_bytes = slab_layout(env->P, nullptr);
+  FX_CREATE(cudaMalloc(&env->slab, env->slab_bytes));
+  FX_CREATE(cudaMemset(env->slab, 0, env->slab_bytes));
+  slab_layout(env->P, env->slab);
   const size_t N = (size_t)c.num_envs;
-  const size_t ring = (c.reward == FX_REWARD_SHARPE) ? (size_t)c.sharpe_window : 1;
-  SlabPlan plan;
-  const size_t capP = (size_t)cap + FXO_SLACK;
-  size_t o_d[9], o_start, o_i[11], o_flags, o_ring, o_welford, o_meta, o_p0, o_p1, o_sz, o_nbar, o_rstats;
-  for (int i = 0; i < 9; i++) o_d[i] = plan.add(N * 8);
-  o_start = plan.add(N * 8);
-  o_nbar = plan.add(N * 6 * 8);
-  o_rstats = plan.add(N * FX_RS_N * 8);
-  for (int i = 0; i < 11; i++) o_i[i] = plan.add(N * 4);
-  o_flags = plan.add(N * 4);
-  o_ring = plan.add(N * ring * 8);
-  o_welford = plan.add(N * FXENV_MAX_FEATURES * 2 * 8);
-  o_meta = plan.add(N * capP * 4);
-  o_p0 = plan.add(N * capP * 8);
-  o_p1 = plan.add(N * capP * 8);
-  o_sz = plan.add(N * capP * 8);
-  const size_t o_ep_lo = plan.add(N * 8), o_ep_span = plan.add(N * 8), o_ep_seed = plan.add(8);
-  const size_t o_ep_begun = plan.add(N * 4), o_ep_done = plan.add(N * 4), o_ep_last = plan.add(N * FXENV_EPISODE_STATS * 8);
-  const size_t o_ep_steps = plan.add(N * 4);
-  env->slab_bytes = plan.bytes;
-  ce = cudaMalloc(&env->slab, plan.bytes);
-  if (ce != cudaSuccess) { fxenv_destroy(env); return cuda_fail(nullptr, ce, "cudaMalloc(state slab)"); }
-  cudaMemset(env->slab, 0, plan.bytes);
-  ce = cudaMalloc(&env->P.seq, (N + 1) * sizeof(int32_t));
-  if (ce != cudaSuccess) { fxenv_destroy(env); return cuda_fail(nullptr, ce, "cudaMalloc(seq)"); }  // frees what was allocated so far
-  cudaMemset(env->P.seq, 0, (N + 1) * sizeof(int32_t));
-  FxDeviceState& st = env->P.st;
-  unsigned char* b = env->slab;
-  double** dcols[9] = {&st.cash, &st.psize, &st.pprice, &st.equity, &st.prev_equity, &st.price,
-                       &st.commission_paid, &st.dd_peak, &st.sub_need};
-  for (int i = 0; i < 9; i++) *dcols[i] = reinterpret_cast<double*>(b + o_d[i]);
-  st.start = reinterpret_cast<int64_t*>(b + o_start);
-  st.nbar = reinterpret_cast<double*>(b + o_nbar);
-  st.rstats = reinterpret_cast<double*>(b + o_rstats);
-  int32_t** icols[11] = {&st.t, &st.total_bars, &st.position, &st.bar_index, &st.trades, &st.n_orders,
-                         &st.sh_len, &st.sh_head, &st.sh_last_step, &st.dd_last_step, &st.n_acc};
-  for (int i = 0; i < 11; i++) *icols[i] = reinterpret_cast<int32_t*>(b + o_i[i]);
-  st.flags = reinterpret_cast<uint32_t*>(b + o_flags);
-  st.sh_ring = reinterpret_cast<double*>(b + o_ring);
-  st.welford = reinterpret_cast<double*>(b + o_welford);
-  st.o_meta = reinterpret_cast<uint32_t*>(b + o_meta);
-  st.o_p0 = reinterpret_cast<double*>(b + o_p0);
-  st.o_p1 = reinterpret_cast<double*>(b + o_p1);
-  st.o_sz = reinterpret_cast<double*>(b + o_sz);
-  st.ep_lo = reinterpret_cast<int64_t*>(b + o_ep_lo);
-  st.ep_span = reinterpret_cast<uint64_t*>(b + o_ep_span);
-  st.ep_seed = reinterpret_cast<uint64_t*>(b + o_ep_seed);
-  st.ep_begun = reinterpret_cast<int32_t*>(b + o_ep_begun);
-  st.ep_done = reinterpret_cast<int32_t*>(b + o_ep_done);
-  st.ep_last = reinterpret_cast<double*>(b + o_ep_last);
-  env->P.ep_steps = reinterpret_cast<int32_t*>(b + o_ep_steps);
+  FX_CREATE(cudaMalloc(&env->P.seq, (N + 1) * sizeof(int32_t)));
+  FX_CREATE(cudaMemset(env->P.seq, 0, (N + 1) * sizeof(int32_t)));
+#undef FX_CREATE
   *out = env;
   return FXENV_OK;
 }
@@ -299,7 +347,6 @@ int fxenv_create(const FxConfig* cfg, FxEnv** out) {
 int fxenv_destroy(FxEnv* env) {
   if (!env) return FXENV_OK;
   DeviceGuard g(env->device);
-  drop_graph(env);
   for (int p = 0; p < FXENV_MAX_PAIRS; p++) {
     cudaFree(env->candles_dev[p]); cudaFree(env->stats_dev[p]); cudaFree(env->minutes_dev[p]);
   }
@@ -324,7 +371,7 @@ int fxenv_load_candles(FxEnv* env, int pair_id, const double* candles_host, int6
   // app/env.py:64-65: the data must be longer than the window
   if (T < (int64_t)c.window_size + 2) return fail(env, FXENV_E_INVALID, "input data is empty or too short for the configured window");
   DeviceGuard g(env->device);
-  drop_graph(env);
+  if (const int rc = params_changing(env)) return rc;  // the table's pointers, tame_data and the LEAN choice change
   cudaFree(env->candles_dev[pair_id]); cudaFree(env->stats_dev[pair_id]); cudaFree(env->minutes_dev[pair_id]);
   env->candles_dev[pair_id] = nullptr; env->stats_dev[pair_id] = nullptr; env->minutes_dev[pair_id] = nullptr;
   env->loaded[pair_id] = false;
@@ -453,35 +500,10 @@ int fxenv_step_many(FxEnv* env, int n_steps, const void* actions_dev, float* obs
     env->launches += 1;
     return FXENV_OK;
   }
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  if (stream != nullptr) cudaStreamIsCapturing(stream, &cs);
-  if (cs != cudaStreamCaptureStatusNone || n_steps == 1 || stream == nullptr) {
-    // already inside someone else's capture (e.g. a torch CUDA graph), or nothing to amortise: plain launches
-    FX_CUDA(env, enqueue(stream));
-    env->launches += n_steps;
-    return FXENV_OK;
-  }
-  FxEnv::CachedGraph* slot = nullptr;
-  for (auto& g : env->graphs)
-    if (g.exec && g.actions == actions_dev && g.obs == obs_dev && g.reward == reward_dev && g.term == terminated_dev &&
-        g.steps == n_steps && g.slots == obs_slots) slot = &g;
-  if (!slot) {
-    slot = (env->graphs[0].used <= env->graphs[1].used) ? &env->graphs[0] : &env->graphs[1];  // least recently used
-    if (slot->exec) { cudaGraphExecDestroy(slot->exec); slot->exec = nullptr; }
-    cudaGraph_t graph = nullptr;
-    FX_CUDA(env, cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
-    cudaError_t e = enqueue(stream);
-    cudaError_t e2 = cudaStreamEndCapture(stream, &graph);
-    if (e != cudaSuccess) { if (graph) cudaGraphDestroy(graph); return cuda_fail(env, e, "capture: fx_launch_step"); }
-    if (e2 != cudaSuccess) return cuda_fail(env, e2, "cudaStreamEndCapture");
-    e = cudaGraphInstantiate(&slot->exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (e != cudaSuccess) { slot->exec = nullptr; return cuda_fail(env, e, "cudaGraphInstantiate"); }
-    slot->actions = actions_dev; slot->obs = obs_dev; slot->reward = reward_dev; slot->term = terminated_dev;
-    slot->steps = n_steps; slot->slots = obs_slots;
-  }
-  slot->used = ++env->graph_clock;
-  FX_CUDA(env, cudaGraphLaunch(slot->exec, stream));
+  // a single step has nothing to amortise: a plain launch
+  const StepManyKey key = {actions_dev, obs_dev, reward_dev, terminated_dev, n_steps, obs_slots};
+  rc = launch_cached(env, env->step_graphs, key, n_steps == 1, stream, enqueue, "capture: fx_launch_step");
+  if (rc) return rc;
   env->launches += n_steps;
   return FXENV_OK;
 }
@@ -588,7 +610,7 @@ int fxenv_set_state(FxEnv* env, const void* buf_host, int64_t nbytes) {
   DeviceGuard g(env->device);
   FX_CUDA(env, cudaDeviceSynchronize());
   FX_CUDA(env, cudaMemcpy(env->slab, static_cast<const char*>(buf_host) + sizeof got, env->slab_bytes, cudaMemcpyHostToDevice));
-  if (env->params_configured) {  // the blob's cash bounds may stem from other per-env costs
+  if (env->deferred & FX_V_PARAMS) {  // the handle has had a table: the blob's cash bounds may stem from other costs
     if (const int rc = invalidate_cash_bounds(env)) return rc;
   }
   env->was_reset = true;
@@ -687,12 +709,8 @@ int fxenv_set_time_limit(FxEnv* env, int32_t max_steps, uint32_t flags) {
   if (flags & ~FXENV_TIME_LIMIT_WINDOW) return fail(env, FXENV_E_INVALID, "unknown time limit flags " + std::to_string(flags));
   DeviceGuard g(env->device);
   if (const int rc = params_changing(env)) return rc;  // also: no count is zeroed while a launch may run
-  if ((max_steps > 0 || flags != 0u) && !env->trunc_configured) {
-    // the truncation kernels' first use on this handle: their attributes, and the persistent grid's minimum over them
-    // (every launch reads the grid and advances the ticket words by its own warp count)
-    FX_CUDA(env, fx_configure_trunc_kernels(env->P));
-    if (env->params_configured) FX_CUDA(env, fx_configure_params_kernels(env->P, FX_V_TRUNC));
-    env->trunc_configured = true;
+  if (max_steps > 0 || flags != 0u) {
+    if (const int rc = use_deferred(env, FX_V_TRUNC)) return rc;
   }
   env->P.max_steps = max_steps;
   env->P.trunc_flags = flags;
@@ -727,7 +745,7 @@ int fxenv_set_env_params(FxEnv* env, const double* params_host) {
   }
   DeviceGuard g(env->device);
   const bool was_on = env->P.env_params_off != 0u;
-  // the kernel choice under the new table: a change of it (or of on / off) drops the graphs captured with the old one
+  // the kernel choice under the new table: a change of it (or of on / off) changes P
   const int lean = lean_choice(env, params_host);
   if (was_on != (params_host != nullptr) || lean != env->P.lean) {
     if (const int rc = params_changing(env)) return rc;
@@ -735,12 +753,7 @@ int fxenv_set_env_params(FxEnv* env, const double* params_host) {
     FX_CUDA(env, cudaDeviceSynchronize());  // no launch may still read the old values
   }
   if (params_host) {
-    if (!env->params_configured) {
-      // the per-env parameter kernels' first use on this handle: their attributes and the persistent grid's minimum
-      FX_CUDA(env, fx_configure_params_kernels(env->P, 0u));
-      if (env->trunc_configured) FX_CUDA(env, fx_configure_params_kernels(env->P, FX_V_TRUNC));
-      env->params_configured = true;
-    }
+    if (const int rc = use_deferred(env, FX_V_PARAMS)) return rc;
     if (!env->params_off) {
       // the first table: the allocation of the sequence words grows by the table (fx_env_params); the words move along
       // (no launch is running: params_changing synchronised)
@@ -847,7 +860,7 @@ struct FxPolicy {
   std::vector<bool> has_weights;       // [members]: set by fxenv_policy_set_member_weights
   int missing_weights = 0;             // members without weights: a rollout needs 0
   bool continuous = false;             // FX_ACTION_CONTINUOUS: Gaussian head, float32 actions (fx_policy_kernel<true>)
-  struct { cudaGraphExec_t exec = nullptr; FxRollout io; uint32_t flags = 0; uint64_t params_epoch = 0; } cached;
+  GraphCache<RolloutKey, 1> graph;     // fxenv_rollout_ex: the last launch sequence, keyed by the FxRollout and the flags
 };
 
 namespace {
@@ -951,7 +964,6 @@ extern "C" {
 int fxenv_policy_destroy(FxPolicy* pol) {
   if (!pol) return FXENV_OK;
   DeviceGuard g(pol->env->device);
-  if (pol->cached.exec) cudaGraphExecDestroy(pol->cached.exec);
   cudaFree(pol->w1); cudaFree(pol->w2); cudaFree(pol->fparams); cudaFree(pol->obs16[0]); cudaFree(pol->obs16[1]);
   cudaFree(pol->h1); cudaFree(pol->head_part); cudaFree(pol->sync);
   cudaFree(pol->scratch_act); cudaFree(pol->scratch_logp);
@@ -1127,34 +1139,13 @@ int fxenv_rollout_ex(FxEnv* env, FxPolicy* pol, const FxRollout* io, uint32_t fl
   if (!io->obs || !io->actions || !io->logp || !io->value || !io->reward || !io->done) return fail(env, FXENV_E_INVALID, "null I/O pointer");
   DeviceGuard g(env->device);
   cudaStream_t stream = (cudaStream_t)stream_;
-  const int64_t nl = 2 * (int64_t)io->horizon + 2;
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  if (stream != nullptr) cudaStreamIsCapturing(stream, &cs);
-  if (cs != cudaStreamCaptureStatusNone || stream == nullptr || (env->P.debug & 32)) {  // inside a capture / legacy stream: plain launches
-    FX_CUDA(env, enqueue_rollout(env, pol, *io, flags, stream));
-    env->launches += nl;
-    return FXENV_OK;
-  }
   // the graph bakes in the buffers, the seed, the flags (greedy or sampling) and the env's kernel parameters (P, by
-  // value: the bracket audit ring): any change re-captures it
-  if (!pol->cached.exec || memcmp(&pol->cached.io, io, sizeof(FxRollout)) != 0 || pol->cached.flags != flags ||
-      pol->cached.params_epoch != env->params_epoch) {
-    if (pol->cached.exec) { cudaGraphExecDestroy(pol->cached.exec); pol->cached.exec = nullptr; }
-    cudaGraph_t graph = nullptr;
-    FX_CUDA(env, cudaStreamBeginCapture(stream, cudaStreamCaptureModeThreadLocal));
-    cudaError_t e = enqueue_rollout(env, pol, *io, flags, stream);
-    cudaError_t e2 = cudaStreamEndCapture(stream, &graph);
-    if (e != cudaSuccess) { if (graph) cudaGraphDestroy(graph); return cuda_fail(env, e, "capture: rollout"); }
-    if (e2 != cudaSuccess) return cuda_fail(env, e2, "cudaStreamEndCapture");
-    e = cudaGraphInstantiate(&pol->cached.exec, graph, 0);
-    cudaGraphDestroy(graph);
-    if (e != cudaSuccess) { pol->cached.exec = nullptr; return cuda_fail(env, e, "cudaGraphInstantiate"); }
-    pol->cached.io = *io;
-    pol->cached.flags = flags;
-    pol->cached.params_epoch = env->params_epoch;
-  }
-  FX_CUDA(env, cudaGraphLaunch(pol->cached.exec, stream));
-  env->launches += nl;
+  // value); FXENV_DEBUG & 32: plain launches (timing experiments)
+  const RolloutKey key = {*io, flags};
+  const auto enqueue = [&](cudaStream_t s) { return enqueue_rollout(env, pol, *io, flags, s); };
+  rc = launch_cached(env, pol->graph, key, (env->P.debug & 32) != 0, stream, enqueue, "capture: rollout");
+  if (rc) return rc;
+  env->launches += 2 * (int64_t)io->horizon + 2;
   return FXENV_OK;
 }
 

@@ -111,14 +111,14 @@ unsigned fx_variant_key(const FxKernelParams& P) {
   return key;
 }
 
-// the kernels of a key: from this translation unit's part of the table, or from the unit that holds the key's half
+// the lookup of each half, indexed by the half's FX_V_TRUNC | FX_V_PARAMS bits: this translation unit's part of the
+// table, then the units that hold the others
+static_assert(FX_V_PARAMS == 2 * FX_V_TRUNC, "a half's index is (key & FX_V_HALF) / FX_V_TRUNC");
+FxEnvKernels (*const half_lookup[4])(int, int, unsigned) = {fx_variant_lookup<0u>, fx_trunc_kernels, fx_params_kernels,
+                                                            fx_params_trunc_kernels};
+
 FxEnvKernels env_kernels(const FxKernelParams& P, unsigned key) {
-  switch (key & (FX_V_TRUNC | FX_V_PARAMS)) {
-    case FX_V_TRUNC: return fx_trunc_kernels(P.cfg.strategy, P.cfg.reward, key);
-    case FX_V_PARAMS: return fx_params_kernels(P.cfg.strategy, P.cfg.reward, key);
-    case FX_V_PARAMS | FX_V_TRUNC: return fx_params_trunc_kernels(P.cfg.strategy, P.cfg.reward, key);
-    default: return fx_variant_lookup<0u>(P.cfg.strategy, P.cfg.reward, key);
-  }
+  return half_lookup[(key & FX_V_HALF) / FX_V_TRUNC](P.cfg.strategy, P.cfg.reward, key);
 }
 
 }  // namespace
@@ -136,7 +136,7 @@ int fx_order_smem_choice(const FxKernelParams& P, int force) {
 // Attributes of one half of the step / rollout instantiations (half: its FX_V_TRUNC | FX_V_PARAMS bits) and the
 // persistent grid: dynamic shared memory above the 48 KB default needs an explicit opt-in per kernel.  P.order_smem is
 // decided.
-static cudaError_t fx_configure_variants(FxKernelParams& P, unsigned half) {
+cudaError_t fx_configure_half(FxKernelParams& P, unsigned half) {
   const size_t smem = step_smem_bytes(P), rsmem = rollout_smem_bytes(P, P.order_smem != 0);
   // ask for enough shared-memory carve-out that FX_MIN_BLOCKS CTAs (+1 KB system use each) fit on an SM
   const int pct = carveout_pct(FX_MIN_BLOCKS, smem);
@@ -165,9 +165,9 @@ static cudaError_t fx_configure_variants(FxKernelParams& P, unsigned half) {
       if (e != cudaSuccess) return e;
     }
     // how many CTAs of the persistent rollout kernel the device holds at once (= its grid size).  The minimum over every
-    // variant configured so far, the bracket audit's and the action repeat's included (the truncation's once a limit is
-    // set): one grid size serves whichever variant a launch picks, so a change that raises those kernels' registers or
-    // shared memory shrinks the grid with them off as well
+    // variant of the halves configured so far, the bracket audit's and the action repeat's included, whatever order the
+    // halves were configured in: one grid size serves whichever variant a launch picks, so a change that raises those
+    // kernels' registers or shared memory shrinks the grid with them off as well
     int per_sm = 0;
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, rk, rcta * 32, rsmem);
     if (e != cudaSuccess) return e;
@@ -187,16 +187,10 @@ cudaError_t fx_configure_kernels(FxKernelParams& P) {
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   P.num_sms = sms > 0 ? sms : 1;
   P.resident_blocks = 0;
-  const cudaError_t e = fx_configure_variants(P, 0u);
+  const cudaError_t e = fx_configure_half(P, 0u);
   if (e != cudaSuccess) return e;
   if (smem <= 48 * 1024) return cudaSuccess;
   return cudaFuncSetAttribute(fx_observe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)observe_smem_bytes(P));
-}
-
-cudaError_t fx_configure_trunc_kernels(FxKernelParams& P) { return fx_configure_variants(P, FX_V_TRUNC); }
-
-cudaError_t fx_configure_params_kernels(FxKernelParams& P, unsigned trunc) {
-  return fx_configure_variants(P, FX_V_PARAMS | (trunc & FX_V_TRUNC));
 }
 
 // The LEAN contract of the specialised kernels (see fx_uses_running_stats): everything here is a property of the

@@ -156,12 +156,9 @@ cudaError_t fx_launch_observe(const FxKernelParams& P, float* obs, cudaStream_t 
                               int stride16 = 0);
 cudaError_t fx_launch_stats(const FxConfig& cfg, const double* candles, double* stats, int64_t T, cudaStream_t stream);
 cudaError_t fx_configure_kernels(FxKernelParams& P);
-// the same for the truncation instantiations; deferred to the first fxenv_set_time_limit that turns truncation on, so
-// that a handle without a time limit never loads their module
-cudaError_t fx_configure_trunc_kernels(FxKernelParams& P);
-// the same for the per-env parameter instantiations (FX_V_PARAMS), with (trunc = FX_V_TRUNC) or without truncation;
-// deferred to the first fxenv_set_env_params
-cudaError_t fx_configure_params_kernels(FxKernelParams& P, unsigned trunc);
+// the same for the kernel half `half` (its FX_V_TRUNC | FX_V_PARAMS bits, see below); the halves with either bit are
+// deferred to the first setter that turns the bit on, so that a handle that never does never loads their modules
+cudaError_t fx_configure_half(FxKernelParams& P, unsigned half);
 // rows_host: the per-env table ([N][FXENV_ENV_PARAMS]) whose costs decide instead of the config's, or nullptr
 bool fx_config_is_lean(const FxKernelParams& P, const double* rows_host = nullptr);
 cudaError_t fx_launch_rollout(const FxKernelParams& P, const void* actions, float* obs, int obs_slots, float* reward,

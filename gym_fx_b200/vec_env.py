@@ -90,6 +90,15 @@ class VecFxEnv:
     def _stream(self) -> int:
         return torch.cuda.current_stream(self.device).cuda_stream
 
+    def _set(self, fn: str, *args):
+        """Call the handle setter `fn` of the library on the handle's device: ValueError with the library's message when
+        it rejects the arguments (FXENV_E_INVALID), FxEnvError on any other failure."""
+        with torch.cuda.device(self.device):
+            rc = getattr(self.L, fn)(self._h, *args)
+        if rc == -1:
+            raise ValueError(self.L.fxenv_last_error(self._h).decode())
+        _native.check(self.L, self._h, rc, fn)
+
     # ------------------------------------------------------------------ Gym-style API
     def reset(self, start_bars: Optional[torch.Tensor] = None, mask: Optional[torch.Tensor] = None):
         """-> (obs [N, D] float32, info).  start_bars: int64 [N] first table row of each env's episode window."""
@@ -331,12 +340,8 @@ class VecFxEnv:
         seed = int(seed)
         if not 0 <= seed < 2**64:
             raise ValueError("seed must be in [0, 2**64)")
-        with torch.cuda.device(self.device):
-            rc = self.L.fxenv_set_reset_starts(self._h, None if lo_a is None else lo_a.ctypes.data,
-                                               None if hi_a is None else hi_a.ctypes.data, seed)
-        if rc == -1:
-            raise ValueError(self.L.fxenv_last_error(self._h).decode())
-        _native.check(self.L, self._h, rc, "fxenv_set_reset_starts")
+        self._set("fxenv_set_reset_starts", None if lo_a is None else lo_a.ctypes.data,
+                  None if hi_a is None else hi_a.ctypes.data, seed)
 
     def _episode_views(self):
         v = self._info_views.get("episodes")
@@ -382,11 +387,7 @@ class VecFxEnv:
         capacity = int(capacity)
         if not 0 <= capacity < 2**31:
             raise ValueError(f"bracket audit capacity must be in [0, 2**31), got {capacity}")
-        with torch.cuda.device(self.device):
-            rc = self.L.fxenv_set_bracket_audit(self._h, capacity)
-        if rc == -1:
-            raise ValueError(self.L.fxenv_last_error(self._h).decode())
-        _native.check(self.L, self._h, rc, "fxenv_set_bracket_audit")
+        self._set("fxenv_set_bracket_audit", capacity)
         self._audit = None
         if capacity:
             p = _native.FxAuditPtrs()
@@ -436,10 +437,7 @@ class VecFxEnv:
         k = int(k)
         if not 1 <= k <= _native.MAX_REPEAT:
             raise ValueError(f"action repeat must be in [1, {_native.MAX_REPEAT}], got {k}")
-        rc = self.L.fxenv_set_action_repeat(self._h, k, _native.REPEAT_HOLD if hold else 0)
-        if rc == -1:
-            raise ValueError(self.L.fxenv_last_error(self._h).decode())
-        _native.check(self.L, self._h, rc, "fxenv_set_action_repeat")
+        self._set("fxenv_set_action_repeat", k, _native.REPEAT_HOLD if hold else 0)
         self.action_repeat = (k, bool(hold))
 
     # ------------------------------------------------------------------ time limit / truncation
@@ -459,11 +457,7 @@ class VecFxEnv:
             raise ValueError(f"time limit must be in [0, 2**31), got {max_steps}")
         if not isinstance(truncate_window, bool):
             raise ValueError(f"truncate_window must be a bool, got {truncate_window!r}")
-        with torch.cuda.device(self.device):
-            rc = self.L.fxenv_set_time_limit(self._h, max_steps, _native.TIME_LIMIT_WINDOW if truncate_window else 0)
-        if rc == -1:
-            raise ValueError(self.L.fxenv_last_error(self._h).decode())
-        _native.check(self.L, self._h, rc, "fxenv_set_time_limit")
+        self._set("fxenv_set_time_limit", max_steps, _native.TIME_LIMIT_WINDOW if truncate_window else 0)
         self.time_limit = (max_steps, truncate_window)
         if max_steps > 0 or truncate_window:
             if self._term_bool is None:
@@ -486,11 +480,7 @@ class VecFxEnv:
         fields = dict(commission=commission, leverage=leverage, slippage=slippage, sl_pips=sl_pips, tp_pips=tp_pips,
                       k_sl=k_sl, k_tp=k_tp)
         table = None if all(v is None for v in fields.values()) else env_params_table(self.cfg, **fields)
-        with torch.cuda.device(self.device):
-            rc = self.L.fxenv_set_env_params(self._h, None if table is None else table.ctypes.data)
-        if rc == -1:
-            raise ValueError(self.L.fxenv_last_error(self._h).decode())
-        _native.check(self.L, self._h, rc, "fxenv_set_env_params")
+        self._set("fxenv_set_env_params", None if table is None else table.ctypes.data)
         self.env_params = table
 
     # ------------------------------------------------------------------ closed loop (policy on the device)

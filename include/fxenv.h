@@ -186,7 +186,9 @@ const char* fxenv_last_error(const FxEnv* env); /* env may be NULL: error of the
  * keeps, app/env.py:62-67, incl. its "too short for the window" ValueError).
  * Copies a host float64 [T, n_cols] row-major candle table (and optional int64 [T] minutes-since-epoch
  * timestamps, needed only by the ATR session filter) to the device, and precomputes the per-bar rolling
- * z-score statistics.  Synchronous. */
+ * z-score statistics.  Synchronous.  A table may be loaded again at any time, in place of the pair's previous one: the
+ * cached step-many graphs and each policy's rollout graph are captured again on their next use, with the new table and
+ * the kernel choice its data make (fxenv_debug_lean). */
 int fxenv_load_candles(FxEnv* env, int pair_id, const double* candles_host, int64_t T, const int64_t* minutes_host);
 
 /* Replaces the observation_space bookkeeping of app/env.py:81-90.
