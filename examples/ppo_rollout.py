@@ -16,6 +16,7 @@ minibatch and advantages are normalised with global statistics (gym_fx_b200.lear
     python examples/ppo_rollout.py --separate-critic --updates 5
     python examples/ppo_rollout.py --randomize-costs 1e-4,3e-4
     python examples/ppo_rollout.py --population 4 --eval-rollouts 2
+    python examples/ppo_rollout.py --obs-norm --updates 5
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 examples/ppo_rollout.py --envs 4096
 
 --action-space continuous trains a Gaussian actor on the Box(-1, 1) action (thresholded to hold / long / short by the
@@ -43,6 +44,10 @@ from seed + m (--seed) with its own optimiser, acts for the m-th contiguous slic
 and one population rollout and one ppo_update_population per update train them all.  The JSON line then also holds
 `members`: per member, the last update's stats and the mean total return of its envs' last finished episodes (and,
 with --eval-rollouts, its greedy evaluation reward).  --envs must be a multiple of 128 x M.
+--obs-norm normalizes the policy's observation with running per-pair statistics (ActorCritic(obs_norm=True),
+learner.ObsNormalizer): seeded from the observation reset() returns, updated from every rollout's observations after
+the PPO update (each member from its own envs), uploaded with the weights; the fused kernels apply them to the bf16
+copy the policy reads.  obs_norm_update_s: the time of one statistics update.
 Prints one JSON line: env-steps/s (decisions) of the rollout phase (policy in the loop) and of the whole train loop, and
 bars/s of the rollout phase as an upper bound (decisions x K: a step that ends an episode runs fewer bars).
 """
@@ -92,6 +97,8 @@ def main():
     ap.add_argument("--population", type=int, default=1,
                     help="policies trained side by side, each on its own slice of the envs (1: one policy)")
     ap.add_argument("--seed", type=int, default=0, help="parameter seed (member m of a population: seed + m)")
+    ap.add_argument("--obs-norm", action="store_true",
+                    help="normalize the policy's observations with running per-pair mean / variance statistics")
     args = ap.parse_args()
     continuous = args.action_space == "continuous"
     cost_max = None
@@ -177,14 +184,20 @@ def main():
     nets = []
     for m in range(M):
         torch.manual_seed(args.seed + m)  # identical replicas on every rank
-        nets.append(ActorCritic(D, hidden=args.hidden, continuous=continuous, separate=args.separate_critic).to(dev))
+        nets.append(ActorCritic(D, hidden=args.hidden, continuous=continuous, separate=args.separate_critic,
+                                obs_norm=args.obs_norm, num_pairs=cfg.num_pairs).to(dev))
     opts = [torch.optim.Adam(n.parameters(), lr=args.lr, eps=1e-5) for n in nets]
     net, opt = nets[0], opts[0]
+    member_envs = [slice(m * N // M, (m + 1) * N // M) for m in range(M)]
+    if args.obs_norm:   # statistics seeded from the current observation (what reset() returned), each member's own envs
+        desc += ", obs-norm (running per-pair statistics)"
+        for m in range(M):
+            nets[m].obs_norm.update(env, env.obs[None], envs=member_envs[m], dist=dist)
     policy = env.make_policy(nets if M > 1 else net)
     buf = None
     prev_done = torch.zeros(N, dtype=torch.uint8, device=dev)
 
-    t_roll = t_upd = 0.0
+    t_roll = t_upd = t_norm = 0.0
     stats = {}
     member_stats = [{} for _ in range(M)]   # a population: the last update's stats of each member
     cost_rng = np.random.default_rng(0xC057 + rank) if cost_max else None
@@ -206,7 +219,15 @@ def main():
         else:
             stats = ppo_update(net, opt, buf, prev_done, dist, epochs=args.epochs, minibatches=args.minibatches)
         prev_done = buf["done"][-1].clone()
-        policy.set_weights(nets if M > 1 else net)        # bf16 repack of the two hidden layers for the next rollout
+        if args.obs_norm:   # after the update, which normalized with the statistics the rollout used
+            torch.cuda.synchronize(dev)
+            tn = time.perf_counter()
+            for m in range(M):
+                nets[m].obs_norm.update(env, buf["obs"][:H], envs=member_envs[m], dist=dist)
+            torch.cuda.synchronize(dev)
+            if it > 0:
+                t_norm += time.perf_counter() - tn
+        policy.set_weights(nets if M > 1 else net)        # bf16 repack of the two hidden layers (and the statistics)
         torch.cuda.synchronize(dev)
         t2 = time.perf_counter()
         if it > 0:                                        # the first iteration pays one-off set-up costs
@@ -278,7 +299,10 @@ def main():
             "hidden": args.hidden, "separate_critic": args.separate_critic, "population": M, "rollout_env_steps_per_s": steps / max(t_roll, 1e-9), "rollout_us_per_step": t_roll / (H * n_it) * 1e6,
             "action_repeat": K, "repeat_mode": args.repeat_mode, "randomize_costs": list(cost_max) if cost_max else None,
             "rollout_bars_per_s_upper_bound": steps * K / max(t_roll, 1e-9),
-            "train_env_steps_per_s": steps / max(t_roll + t_upd, 1e-9), "update_s": t_upd / n_it, **stats,
+            "train_env_steps_per_s": steps / max(t_roll + t_upd, 1e-9), "update_s": t_upd / n_it,
+            "obs_norm": args.obs_norm, "obs_norm_update_s": t_norm / n_it if args.obs_norm else None,
+            "obs_norm_finite": all(bool(torch.isfinite(n.obs_norm.mean).all() and torch.isfinite(n.obs_norm.var).all())
+                                   for n in nets) if args.obs_norm else None, **stats,
             **({"members": members} if M > 1 else {})}), flush=True)
     env.close()
     if dist:

@@ -860,6 +860,11 @@ struct FxPolicy {
   std::vector<bool> has_weights;       // [members]: set by fxenv_policy_set_member_weights
   int missing_weights = 0;             // members without weights: a rollout needs 0
   bool continuous = false;             // FX_ACTION_CONTINUOUS: Gaussian head, float32 actions (fx_policy_kernel<true>)
+  // observation normalizer (fxenv_policy_set_obs_norm), allocated by its first use: mean [members][num_pairs][k_pad] |
+  // rstd [same] | clip [members], the pad columns zero
+  float* norm = nullptr;
+  std::vector<bool> norm_on;           // [members]
+  int norm_members = 0;                // members with a normalizer: a rollout needs 0 or all
   GraphCache<RolloutKey, 1> graph;     // fxenv_rollout_ex: the last launch sequence, keyed by the FxRollout and the flags
 };
 
@@ -911,7 +916,12 @@ cudaError_t enqueue_rollout(FxEnv* env, FxPolicy* pol, const FxRollout& io, uint
   const bool tile_sync = !skip && !pol->separate && tsv && atoi(tsv) != 0;
   cudaError_t e = cudaMemsetAsync(pol->sync, 0, (2 * (size_t)pol->tiles + 1) * sizeof(int32_t), s);
   if (e != cudaSuccess) return e;
-  e = fx_launch_observe(env->P, io.obs, s, pol->obs16[0], pol->k_pad);  // the current observation, both copies
+  // with a normalizer on, the bf16 copies are the normalized ones (fx_observe_norm_kernel, fx_step_norm_kernel)
+  const size_t MPK = (size_t)pol->members * (size_t)env->P.cfg.num_pairs * (size_t)pol->k_pad;
+  const FxObsNorm norm = {pol->norm, pol->norm + MPK, pol->norm + 2 * MPK, (int32_t)(N / (size_t)pol->members),
+                          env->P.cfg.num_pairs};
+  const FxObsNorm* nm = pol->norm_members > 0 ? &norm : nullptr;
+  e = fx_launch_observe(env->P, io.obs, s, pol->obs16[0], pol->k_pad, nm);  // the current observation, both copies
   if (e != cudaSuccess) return e;
   int groups = (int)(N / 2048);  // measured (H100 SXM, 4096 envs, cfg4 shape), us/step: 46.6 with 1 group, 44.8 with 2, 46.4 with 4
   if (groups > FxPolicy::kGroups) groups = FxPolicy::kGroups;
@@ -944,7 +954,7 @@ cudaError_t enqueue_rollout(FxEnv* env, FxPolicy* pol, const FxRollout& io, uint
       if (!(skip & 1))
       e = fx_launch_step(env->P, actions + (size_t)t * N, io.obs + (size_t)((t + 1) % slots) * N * D, io.reward + (size_t)t * N,
                          nullptr, io.done + (size_t)t * N, sg, (int)e0, (int)e1, pol->obs16[(t + 1) & 1], pol->k_pad,
-                         tile_sync ? &ts : nullptr);
+                         tile_sync ? &ts : nullptr, nm);
       if (e != cudaSuccess) return e;
     }
     if (g > 0) {
@@ -966,7 +976,7 @@ int fxenv_policy_destroy(FxPolicy* pol) {
   DeviceGuard g(pol->env->device);
   cudaFree(pol->w1); cudaFree(pol->w2); cudaFree(pol->fparams); cudaFree(pol->obs16[0]); cudaFree(pol->obs16[1]);
   cudaFree(pol->h1); cudaFree(pol->head_part); cudaFree(pol->sync);
-  cudaFree(pol->scratch_act); cudaFree(pol->scratch_logp);
+  cudaFree(pol->scratch_act); cudaFree(pol->scratch_logp); cudaFree(pol->norm);
   for (auto& st : pol->side) if (st) cudaStreamDestroy(st);
   if (pol->ev_fork) cudaEventDestroy(pol->ev_fork);
   for (auto& ev : pol->ev_join) if (ev) cudaEventDestroy(ev);
@@ -1040,6 +1050,7 @@ int fxenv_policy_create_ex3(FxEnv* env, int32_t hidden, uint32_t flags, int32_t 
   pol->nets = pol->separate ? 2 : 1;
   pol->members = members;
   pol->has_weights.assign((size_t)members, false);
+  pol->norm_on.assign((size_t)members, false);
   pol->missing_weights = members;
   const size_t N = (size_t)env->P.cfg.num_envs, D = (size_t)env->P.obs_dim, M = (size_t)members;
   pol->k_pad = (int)((D + 63) / 64 * 64);
@@ -1119,6 +1130,59 @@ int fxenv_policy_set_member_weights(FxPolicy* pol, int32_t member, const FxPolic
   return FXENV_OK;
 }
 
+int fxenv_policy_set_obs_norm(FxPolicy* pol, int32_t member, const float* mean_dev, const float* rstd_dev, float clip,
+                              void* stream_) {
+  if (!pol) return FXENV_E_INVALID;
+  FxEnv* env = pol->env;
+  if (member < 0 || member >= pol->members)
+    return fail(env, FXENV_E_INVALID, "policy member " + std::to_string(member) + " out of range [0, " +
+                                      std::to_string(pol->members) + ")");
+  if ((mean_dev == nullptr) != (rstd_dev == nullptr))
+    return fail(env, FXENV_E_INVALID, "fxenv_policy_set_obs_norm: mean and rstd must both be given or both be NULL");
+  const size_t m = (size_t)member;
+  const bool on = mean_dev != nullptr;
+  if (on && !(clip > 0.0f))  // also NaN
+    return fail(env, FXENV_E_INVALID, "fxenv_policy_set_obs_norm: clip must be > 0 (+inf allowed), got " + std::to_string(clip));
+  DeviceGuard g(env->device);
+  cudaStream_t s = (cudaStream_t)stream_;
+  const size_t P = (size_t)env->P.cfg.num_pairs, D = (size_t)env->P.obs_dim, KP = (size_t)pol->k_pad;
+  const size_t MPK = (size_t)pol->members * P * KP;
+  if (on && !pol->norm) {  // zeroed once: the pad columns stay 0
+    FX_CUDA(env, cudaMalloc(&pol->norm, (2 * MPK + (size_t)pol->members) * sizeof(float)));
+    FX_CUDA(env, cudaMemset(pol->norm, 0, (2 * MPK + (size_t)pol->members) * sizeof(float)));
+  }
+  if (on != pol->norm_on[m]) {  // another kernel variant: the cached rollout graph is captured again
+    if (const int rc = params_changing(env)) return rc;
+  }
+  if (on) {
+    float* mean = pol->norm + m * P * KP;
+    FX_CUDA(env, cudaMemcpy2DAsync(mean, KP * 4, mean_dev, D * 4, D * 4, P, cudaMemcpyDeviceToDevice, s));
+    FX_CUDA(env, cudaMemcpy2DAsync(mean + MPK, KP * 4, rstd_dev, D * 4, D * 4, P, cudaMemcpyDeviceToDevice, s));
+    FX_CUDA(env, cudaMemcpyAsync(pol->norm + 2 * MPK + m, &clip, sizeof(float), cudaMemcpyHostToDevice, s));
+  }
+  if (on != pol->norm_on[m]) {
+    pol->norm_on[m] = on;
+    pol->norm_members += on ? 1 : -1;
+  }
+  return FXENV_OK;
+}
+
+int fxenv_obs_moments(FxEnv* env, const float* obs_dev, int32_t slots, int32_t env_begin, int32_t env_end,
+                      const float* shift_dev, double* out_dev, void* stream_) {
+  if (!env) return FXENV_E_INVALID;
+  if (!obs_dev || !shift_dev || !out_dev) return fail(env, FXENV_E_INVALID, "fxenv_obs_moments: null pointer");
+  const int N = env->P.cfg.num_envs;
+  if (slots < 1) return fail(env, FXENV_E_INVALID, "fxenv_obs_moments: slots must be >= 1, got " + std::to_string(slots));
+  if (env_begin < 0 || env_end > N || env_begin >= env_end)
+    return fail(env, FXENV_E_INVALID, "fxenv_obs_moments: env range [" + std::to_string(env_begin) + ", " +
+                                      std::to_string(env_end) + ") is empty or outside [0, " + std::to_string(N) + ")");
+  DeviceGuard g(env->device);
+  FX_CUDA(env, fx_launch_obs_moments(obs_dev, slots, N, env->P.obs_dim, env->P.cfg.num_pairs, env_begin, env_end, shift_dev,
+                                     out_dev, (cudaStream_t)stream_));
+  env->launches += 2;
+  return FXENV_OK;
+}
+
 int fxenv_rollout(FxEnv* env, FxPolicy* pol, const FxRollout* io, void* stream_) {
   return fxenv_rollout_ex(env, pol, io, 0u, stream_);
 }
@@ -1135,6 +1199,9 @@ int fxenv_rollout_ex(FxEnv* env, FxPolicy* pol, const FxRollout* io, uint32_t fl
     return fail(env, FXENV_E_STATE, std::to_string(pol->missing_weights) + " of " + std::to_string(pol->members) +
                                     " policy members have no weights yet (first: member " + std::to_string(first) + ")");
   }
+  if (pol->norm_members > 0 && pol->norm_members < pol->members)
+    return fail(env, FXENV_E_STATE, std::to_string(pol->norm_members) + " of " + std::to_string(pol->members) +
+                                    " policy members have an observation normalizer: every member or none");
   if (io->horizon < 1 || io->obs_slots < 2) return fail(env, FXENV_E_INVALID, "horizon must be >= 1 and obs_slots >= 2");
   if (!io->obs || !io->actions || !io->logp || !io->value || !io->reward || !io->done) return fail(env, FXENV_E_INVALID, "null I/O pointer");
   DeviceGuard g(env->device);

@@ -340,6 +340,41 @@ __device__ __forceinline__ void fx_st16x4(uint16_t* o16, int j, float4 v) {  // 
   }
 }
 
+// The normalized bf16 copy (FxObsNorm, the fx_step_norm_kernel / fx_observe_norm_kernel variants): the env's row of the
+// copy with its row of statistics and its clip.  The emit paths take either sink through the same fx_st16 / fx_st16x4
+// calls; a plain uint16_t* keeps its __restrict__ (FxSink), so the plain kernels compile as before.
+struct FxRow16N {
+  uint16_t* p;
+  const float* mean;
+  const float* rstd;
+  float clip;
+};
+template <class R16> struct FxSink { typedef R16 T; };
+template <> struct FxSink<uint16_t*> { typedef uint16_t* __restrict__ T; };
+
+__device__ __forceinline__ FxRow16N fx_norm_row(const FxObsNorm& nm, uint16_t* obs16, int stride16, int env) {
+  const int m = env / nm.member_envs, p = env % nm.num_pairs;
+  const size_t off = ((size_t)m * (size_t)nm.num_pairs + (size_t)p) * (size_t)stride16;
+  return FxRow16N{obs16 + (size_t)env * (size_t)stride16, nm.mean + off, nm.rstd + off, __ldg(nm.clip + m)};
+}
+// (x - mean) * rstd clamped to [-clip, clip]: each operation rounded in float32 (the build does not contract), a NaN
+// passes through -- torch's clamp((x - mean) * rstd, -clip, clip), bit for bit
+__device__ __forceinline__ float fx_norm1(float x, float m, float r, float c) {
+  const float t = (x - m) * r;
+  return t < -c ? -c : (t > c ? c : t);
+}
+__device__ __forceinline__ void fx_st16(const FxRow16N& o, int j, float v) {
+  if (o.p) fx_st16(o.p, j, fx_norm1(v, __ldg(o.mean + j), __ldg(o.rstd + j), o.clip));
+}
+__device__ __forceinline__ void fx_st16x4(const FxRow16N& o, int j, float4 v) {  // the statistics row is 16-byte aligned
+  if (o.p) {
+    const float4 m = __ldg(reinterpret_cast<const float4*>(o.mean + j)), r = __ldg(reinterpret_cast<const float4*>(o.rstd + j));
+    v.x = fx_norm1(v.x, m.x, r.x, o.clip); v.y = fx_norm1(v.y, m.y, r.y, o.clip);
+    v.z = fx_norm1(v.z, m.z, r.z, o.clip); v.w = fx_norm1(v.w, m.w, r.w, o.clip);
+    fx_st16x4(o.p, j, v);
+  }
+}
+
 // ---- observation windows: preprocessor.make_observation (features | prices | returns) in the flat VecEnv layout ----
 // `win` = the staged rows [left, s) (shift already applied): element (k, col) at win[k * C + col].
 // float32 finishing of one feature value: np.clip then np.nan_to_num (feature_window_preprocessor.py:119-123)
@@ -353,11 +388,11 @@ __device__ __forceinline__ float fx_finish_t(float v, float clipf) {
 }
 
 // LONG: windows of several hundred rows, where loop overhead outweighs instruction-cache footprint (the loops are unrolled)
-template <bool FAST5, bool CLIP, bool TAME, bool LONG, bool O16>
+template <bool FAST5, bool CLIP, bool TAME, bool LONG, bool O16, class R16>
 __device__ __noinline__ void fx_emit_windows_t(const FxKernelParams& P, int lane, int s, bool scale,
                                                const double* __restrict__ win, const double* sstat,
-                                               float* __restrict__ out, uint16_t* __restrict__ o16_) {
-  uint16_t* __restrict__ const o16 = O16 ? o16_ : nullptr;  // O16 == false: the bf16 copy is compiled out
+                                               float* __restrict__ out, typename FxSink<R16>::T o16_) {
+  const typename FxSink<R16>::T o16 = O16 ? o16_ : R16{};  // O16 == false: the bf16 copy is compiled out
   const FxConfig& c = P.cfg;
   const int W = c.window_size, C = c.n_cols;
   int left = s - W;
@@ -459,12 +494,12 @@ __device__ __noinline__ void fx_emit_windows_t(const FxKernelParams& P, int lane
 // What it needs of the configuration arrives BY VALUE: as a non-inlined function taking a reference to the kernel parameters
 // it read them with generic loads (a constant-bank address formed at run time), ~10 dependent round trips at the top of
 // every row.  (It is now inlined as well.)  NOBIN: no binary pass-through feature (LEAN contract).
-template <bool CLIP, bool TAME, bool O16, bool PAD, bool LONG, bool NOBIN>
+template <bool CLIP, bool TAME, bool O16, bool PAD, bool LONG, bool NOBIN, class R16>
 __device__ __forceinline__ void fx_emit_fast5_q(const int lane, const bool scale, const double* __restrict__ win,
-                                             const double* sstat, float* __restrict__ out, uint16_t* __restrict__ o16_,
+                                             const double* sstat, float* __restrict__ out, typename FxSink<R16>::T o16_,
                                              const int pad, const int W, const float clipf, const int pc,
                                              const unsigned binary_mask) {
-  uint16_t* __restrict__ const o16 = O16 ? o16_ : nullptr;
+  const typename FxSink<R16>::T o16 = O16 ? o16_ : R16{};
   const int pad5 = 5 * pad;
   if (lane < 30) {
     const int l5 = lane % 5;
@@ -527,20 +562,20 @@ __device__ __forceinline__ void fx_emit_fast5_q(const int lane, const bool scale
   }
 }
 
-template <bool FAST5, bool O16 = true, bool LEAN = false>
+template <bool FAST5, bool O16 = true, bool LEAN = false, class R16 = uint16_t*>
 __device__ __forceinline__ void fx_emit_windows(const FxKernelParams& P, int lane, int s, bool scale,
                                                 const double* __restrict__ win, const double* sstat,
-                                                float* __restrict__ out, uint16_t* __restrict__ o16 = nullptr) {
+                                                float* __restrict__ out, typename FxSink<R16>::T o16 = R16{}) {
   const int pad = P.cfg.window_size - s;  // > 0: the first rows of the window repeat the episode's first bar
   if (LEAN) {  // window % 4 == 0, price window, clip > 0 and finite data are part of the LEAN contract
     if ((reinterpret_cast<uintptr_t>(out) & 15) == 0) {
       const int W = P.cfg.window_size, pc = P.cfg.price_col;
       const float clipf = (float)P.cfg.feature_clip;
-      if (pad > 0) fx_emit_fast5_q<true, true, O16, true, false, true>(lane, scale, win, sstat, out, o16, pad, W, clipf, pc, 0u);
-      else if (W >= FX_LONG_MIN_W) fx_emit_fast5_q<true, true, O16, false, true, true>(lane, scale, win, sstat, out, o16, 0, W, clipf, pc, 0u);
-      else fx_emit_fast5_q<true, true, O16, false, false, true>(lane, scale, win, sstat, out, o16, 0, W, clipf, pc, 0u);
+      if (pad > 0) fx_emit_fast5_q<true, true, O16, true, false, true, R16>(lane, scale, win, sstat, out, o16, pad, W, clipf, pc, 0u);
+      else if (W >= FX_LONG_MIN_W) fx_emit_fast5_q<true, true, O16, false, true, true, R16>(lane, scale, win, sstat, out, o16, 0, W, clipf, pc, 0u);
+      else fx_emit_fast5_q<true, true, O16, false, false, true, R16>(lane, scale, win, sstat, out, o16, 0, W, clipf, pc, 0u);
     } else {
-      fx_emit_windows_t<true, true, true, false, O16>(P, lane, s, scale, win, sstat, out, o16);
+      fx_emit_windows_t<true, true, true, false, O16, R16>(P, lane, s, scale, win, sstat, out, o16);
     }
     return;
   }
@@ -553,29 +588,29 @@ __device__ __forceinline__ void fx_emit_windows(const FxKernelParams& P, int lan
 #pragma unroll
       for (int f = 0; f < 5; f++) bm |= P.cfg.feature_binary[f] ? (1u << f) : 0u;
     }
-    if (pad > 0) fx_emit_fast5_q<true, true, O16, true, false, false>(lane, scale, win, sstat, out, o16, pad, W, clipf, pc, bm);
-    else if (W >= FX_LONG_MIN_W) fx_emit_fast5_q<true, true, O16, false, true, false>(lane, scale, win, sstat, out, o16, 0, W, clipf, pc, bm);
-    else fx_emit_fast5_q<true, true, O16, false, false, false>(lane, scale, win, sstat, out, o16, 0, W, clipf, pc, bm);
+    if (pad > 0) fx_emit_fast5_q<true, true, O16, true, false, false, R16>(lane, scale, win, sstat, out, o16, pad, W, clipf, pc, bm);
+    else if (W >= FX_LONG_MIN_W) fx_emit_fast5_q<true, true, O16, false, true, false, R16>(lane, scale, win, sstat, out, o16, 0, W, clipf, pc, bm);
+    else fx_emit_fast5_q<true, true, O16, false, false, false, R16>(lane, scale, win, sstat, out, o16, 0, W, clipf, pc, bm);
     return;
   }
   const bool lng = P.cfg.window_size >= 384;
   if (P.cfg.feature_clip > 0.0) {
     if (P.tame_data) {
-      if (lng) fx_emit_windows_t<FAST5, true, true, true, O16>(P, lane, s, scale, win, sstat, out, o16);
-      else fx_emit_windows_t<FAST5, true, true, false, O16>(P, lane, s, scale, win, sstat, out, o16);
+      if (lng) fx_emit_windows_t<FAST5, true, true, true, O16, R16>(P, lane, s, scale, win, sstat, out, o16);
+      else fx_emit_windows_t<FAST5, true, true, false, O16, R16>(P, lane, s, scale, win, sstat, out, o16);
     } else {
-      fx_emit_windows_t<FAST5, true, false, false, O16>(P, lane, s, scale, win, sstat, out, o16);
+      fx_emit_windows_t<FAST5, true, false, false, O16, R16>(P, lane, s, scale, win, sstat, out, o16);
     }
   } else {
-    fx_emit_windows_t<FAST5, false, false, false, O16>(P, lane, s, scale, win, sstat, out, o16);
+    fx_emit_windows_t<FAST5, false, false, false, O16, R16>(P, lane, s, scale, win, sstat, out, o16);
   }
 }
 
 // issue + wait + emit in one go (terminated path, observe kernel)
-template <bool FAST5>
+template <bool FAST5, class R16 = uint16_t*>
 __device__ __forceinline__ void fx_stream_windows(const FxKernelParams& P, const FxPairTable& tb, int env, int lane, int s,
                                                   int64_t start, const WarpSmem& ws, float* __restrict__ out,
-                                                  uint16_t* __restrict__ o16 = nullptr) {
+                                                  typename FxSink<R16>::T o16 = R16{}) {
   const int W = P.cfg.window_size;
   int left = s - W;
   if (left < 0) left = 0;
@@ -584,7 +619,7 @@ __device__ __forceinline__ void fx_stream_windows(const FxKernelParams& P, const
   const int shift = fx_window_issue(tb, P.cfg.n_cols, start, left, s - left, lane, ws);
   const bool scale = fx_prepare_stats(P, tb, env, lane, s, start, ws.stat);
   fx_window_wait(ws);
-  fx_emit_windows<FAST5>(P, lane, s, scale, ws.win + shift, ws.stat, out, o16);
+  fx_emit_windows<FAST5, true, false, R16>(P, lane, s, scale, ws.win + shift, ws.stat, out, o16);
 }
 
 __device__ __forceinline__ int fx_scalar_offset(const FxConfig& c) {
@@ -595,9 +630,9 @@ __device__ __forceinline__ int fx_scalar_offset(const FxConfig& c) {
 
 // the 4 agent scalars at the end of the row (one lane)
 // `last` = price_column of the last window row (local row bar_index - 1)
-template <bool LEAN = false>
+template <bool LEAN = false, class R16 = uint16_t*>
 __device__ __forceinline__ void fx_write_scalars(const FxKernelParams& P, const FxEnvRegs& e, int32_t total_bars,
-                                                 double last, float* __restrict__ out, uint16_t* __restrict__ o16 = nullptr) {
+                                                 double last, float* __restrict__ out, typename FxSink<R16>::T o16 = R16{}) {
   const FxConfig& c = P.cfg;
   const bool inc_agent = LEAN || (c.preproc == FX_PREPROC_DEFAULT) || c.include_agent_state;
   if (!inc_agent) return;
@@ -732,9 +767,11 @@ __device__ __forceinline__ size_t fx_out_idx(const FxStepOut& o, int env) { retu
 __device__ __forceinline__ float* fx_obs_row(const FxKernelParams& P, const FxStepOut& o, int env) {
   return o.obs + ((size_t)o.obs_slot_row + (size_t)env) * (size_t)P.obs_dim;
 }
-template <bool O16>
-__device__ __forceinline__ uint16_t* fx_obs_row16(const FxStepOut& o, int env) {
-  return (O16 && o.obs16) ? o.obs16 + (size_t)env * (size_t)o.stride16 : nullptr;
+// NORM: the normalized copy's sink (FxRow16N) of the env
+template <bool O16, bool NORM = false>
+__device__ __forceinline__ auto fx_obs_row16(const FxStepOut& o, int env, const FxObsNorm* norm) {
+  if constexpr (NORM) return fx_norm_row(*norm, o.obs16, o.stride16, env);
+  else return (O16 && o.obs16) ? o.obs16 + (size_t)env * (size_t)o.stride16 : nullptr;
 }
 
 // Phase stamps of the timing build (make TIMING=1, tools/phase_timing.py): lane 0 writes stamp i of the env's FX_NSTAMP
@@ -930,16 +967,20 @@ __device__ __forceinline__ double fx_step_reward(const FxKernelParams& P, const 
 // RESIDENT (with CARRY): the env's order table lives in ws.op0/op1/osz/ometa while the carry record is valid -- loaded
 // from global memory by a step without carry_in, written back by a step that returns false (terminated branch) and by
 // the caller at the end of its ticket (fx_rollout_kernel).
+// NORM (with O16): the bf16 copy is the normalized one of `norm` (FxObsNorm).
 // REPEAT (with CARRY): the call is substep sub->j of a step.  A substep that does not end the step issues no window
 // copy, stages no statistics and stores no row, reward or flag (the running Welford statistics still advance); it adds
 // its reward to sub->racc and leaves the carry record for the next substep.
-template <int STRATEGY, int REWARD, unsigned V, bool O16, bool CARRY = false>
+template <int STRATEGY, int REWARD, unsigned V, bool O16, bool CARRY = false, bool NORM = false>
 __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void* __restrict__ actions, float* __restrict__ obs,
                                             float* __restrict__ reward, double* __restrict__ reward64,
                                             uint8_t* __restrict__ terminated, const int env, const int lane, const WarpSmem& ws,
                                             const unsigned phase = 0u, const unsigned step_row = 0u, const unsigned obs_slot_row = 0u,
                                             uint16_t* __restrict__ obs16 = nullptr, const int stride16 = 0,
-                                            const bool carry_in = false, FxSubstep* sub = nullptr) {
+                                            const bool carry_in = false, FxSubstep* sub = nullptr,
+                                            const FxObsNorm* norm = nullptr) {
+  static_assert(!NORM || O16, "the normalizer applies to the bf16 copy");
+  typedef decltype(fx_obs_row16<O16, NORM>(FxStepOut{}, 0, nullptr)) R16;
   const FxStepOut o{obs, obs16, reward, reward64, terminated, step_row, obs_slot_row, stride16};
   constexpr bool FAST5 = (V & FX_V_FAST5) != 0, LEAN = (V & FX_V_LEAN) != 0, RESIDENT = (V & FX_V_RESIDENT) != 0;
   constexpr bool AUDIT = (V & FX_V_AUDIT) != 0, REPEAT = (V & FX_V_REPEAT) != 0, TRUNC = (V & FX_V_TRUNC) != 0;
@@ -1019,7 +1060,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       o.reward[fx_out_idx(o, env)] = 0.0f;
       if (o.reward64) o.reward64[fx_out_idx(o, env)] = 0.0;
       o.terminated[fx_out_idx(o, env)] = c.auto_reset ? 0 : ((TRUNC && !(flags & FX_FLAG_TERMINATED)) ? FXENV_DONE_TRUNCATED : 1);
-      fx_write_scalars<LEAN>(P, e, total_bars, tb.candles[(start + e.bar_index - 1) * (int64_t)C + c.price_col], fx_obs_row(P, o, env), fx_obs_row16<O16>(o, env));
+      fx_write_scalars<LEAN, R16>(P, e, total_bars, tb.candles[(start + e.bar_index - 1) * (int64_t)C + c.price_col], fx_obs_row(P, o, env), fx_obs_row16<O16, NORM>(o, env, norm));
     }
     {
       const int s = e.bar_index;
@@ -1029,7 +1070,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
       const int shift = fx_window_issue(tb, C, start, left, s - left, lane, ws);
       const bool scale = fx_prepare_stats(P, tb, env, lane, s, start, ws.stat);
       fx_window_wait(ws, phase);
-      fx_emit_windows<FAST5, O16, LEAN>(P, lane, s, scale, ws.win + shift, ws.stat, fx_obs_row(P, o, env), fx_obs_row16<O16>(o, env));
+      fx_emit_windows<FAST5, O16, LEAN, R16>(P, lane, s, scale, ws.win + shift, ws.stat, fx_obs_row(P, o, env), fx_obs_row16<O16, NORM>(o, env, norm));
     }
     if (REPEAT) sub->ended = true;  // rule 1 of the repeat: a terminated env runs this one substep
     return false;  // (the carry record does not follow resets / ended episodes: the next step reloads the arrays)
@@ -1263,7 +1304,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
         o.reward[fx_out_idx(o, env)] = (float)r;
         if (o.reward64) o.reward64[fx_out_idx(o, env)] = r;
         o.terminated[fx_out_idx(o, env)] = term ? 1 : ((TRUNC && trunc) ? FXENV_DONE_TRUNCATED : 0);
-        fx_write_scalars<LEAN>(P, e, total_bars, last_price, fx_obs_row(P, o, env), fx_obs_row16<O16>(o, env));
+        fx_write_scalars<LEAN, R16>(P, e, total_bars, last_price, fx_obs_row(P, o, env), fx_obs_row16<O16, NORM>(o, env, norm));
       }
       if (CARRY) {  // what the env's next step starts from, should this warp run it (the arrays above stay authoritative)
         double* __restrict__ cr = ws.carry;
@@ -1312,7 +1353,7 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
   __syncwarp();
   if ((!REPEAT || emit) && !(dbg & 1)) {
     fx_window_wait(ws, phase);
-    fx_emit_windows<FAST5, O16, LEAN>(P, lane, s_obs, scale, ws.win + win_shift, ws.stat, fx_obs_row(P, o, env), fx_obs_row16<O16>(o, env));
+    fx_emit_windows<FAST5, O16, LEAN, R16>(P, lane, s_obs, scale, ws.win + win_shift, ws.stat, fx_obs_row(P, o, env), fx_obs_row16<O16, NORM>(o, env, norm));
   }
   if (lane < 5 && !(dbg & 2)) st.nbar[(int64_t)env * 6 + lane] = nbar_next;
   if (CARRY) {
@@ -1328,19 +1369,20 @@ __device__ __forceinline__ bool fx_step_env(const FxKernelParams& P, const void*
 // One step of up to P.repeat substeps (the REPEAT instantiations): substeps run until one ends the step.  They hand the
 // env to each other through the carry record (RESIDENT: and the shared copy of the order table), so only the first one
 // loads it from global memory.  Returns what the last substep returned.
-template <int STRATEGY, int REWARD, unsigned V, bool O16>
+template <int STRATEGY, int REWARD, unsigned V, bool O16, bool NORM = false>
 __device__ __forceinline__ bool fx_step_repeat(const FxKernelParams& P, const void* __restrict__ actions, float* __restrict__ obs,
                                                float* __restrict__ reward, double* __restrict__ reward64,
                                                uint8_t* __restrict__ terminated, const int env, const int lane, const WarpSmem& ws,
                                                const unsigned phase, const unsigned step_row, const unsigned obs_slot_row,
-                                               uint16_t* __restrict__ obs16, const int stride16, bool carry) {
+                                               uint16_t* __restrict__ obs16, const int stride16, bool carry,
+                                               const FxObsNorm* norm = nullptr) {
   FxSubstep sub;
   sub.racc = 0.0;
   sub.ended = false;
 #pragma unroll 1
   for (sub.j = 0;; ++sub.j) {
-    carry = fx_step_env<STRATEGY, REWARD, V, O16, true>(P, actions, obs, reward, reward64, terminated, env, lane, ws, phase,
-                                                        step_row, obs_slot_row, obs16, stride16, carry, &sub);
+    carry = fx_step_env<STRATEGY, REWARD, V, O16, true, NORM>(P, actions, obs, reward, reward64, terminated, env, lane, ws, phase,
+                                                              step_row, obs_slot_row, obs16, stride16, carry, &sub, norm);
     if (sub.ended) break;
     __syncwarp();  // the substep's stores (state arrays, carry record) before the next substep's loads
   }
@@ -1360,11 +1402,13 @@ __device__ __forceinline__ void fx_st_release(int32_t* p, int v) {
 // the NEXT kernel of the stream / graph may be scheduled while this grid drains (its CTAs take SM slots as ours exit and
 // park at their own griddepcontrol.wait), which hides the launch gap between dependent steps.  Everything that touches
 // memory written by the previous kernel comes after the wait.
-template <int STRATEGY, int REWARD, unsigned V>
-__global__ void __launch_bounds__(FX_WARPS * 32, FX_MIN_BLOCKS)
-fx_step_kernel(const __grid_constant__ FxKernelParams P, const void* __restrict__ actions, float* __restrict__ obs,
-               float* __restrict__ reward, double* __restrict__ reward64, uint8_t* __restrict__ terminated,
-               const int env_begin, const int env_end, uint16_t* __restrict__ obs16, const int stride16, const FxTileSync sync) {
+// NORM: fx_step_norm_kernel, the normalized bf16 copy of `norm` (obs16 is then never nullptr).
+template <int STRATEGY, int REWARD, unsigned V, bool NORM>
+__device__ __forceinline__ void
+fx_step_kernel_body(const FxKernelParams& P, const void* __restrict__ actions, float* __restrict__ obs,
+                    float* __restrict__ reward, double* __restrict__ reward64, uint8_t* __restrict__ terminated,
+                    const int env_begin, const int env_end, uint16_t* __restrict__ obs16, const int stride16,
+                    const FxTileSync& sync, const FxObsNorm* norm) {
   static_assert((V & FX_V_RESIDENT) == 0, "the step kernel keeps no order table in shared memory");
   extern __shared__ __align__(16) unsigned char fx_smem[];
   const FxConfig& c = P.cfg;
@@ -1402,7 +1446,13 @@ fx_step_kernel(const __grid_constant__ FxKernelParams P, const void* __restrict_
   if (klog) { long long g1; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g1)); klog[2] = g1; }
 #endif
   // the bf16 copy of the row (closed loop only) is a compile-time variant: no per-store pointer tests in the plain step
-  if constexpr ((V & FX_V_REPEAT) != 0) {  // action repeat: the step's substeps (the emitting one writes both rows)
+  if constexpr (NORM) {
+    if constexpr ((V & FX_V_REPEAT) != 0)
+      fx_step_repeat<STRATEGY, REWARD, V, true, true>(P, actions, obs, reward, reward64, terminated, env, lane, ws, 0u, 0u, 0u, obs16, stride16, false, norm);
+    else
+      fx_step_env<STRATEGY, REWARD, V, true, false, true>(P, actions, obs, reward, reward64, terminated, env, lane, ws, 0u, 0u, 0u, obs16, stride16,
+                                                          false, nullptr, norm);
+  } else if constexpr ((V & FX_V_REPEAT) != 0) {  // action repeat: the step's substeps (the emitting one writes both rows)
     if (obs16) fx_step_repeat<STRATEGY, REWARD, V, true>(P, actions, obs, reward, reward64, terminated, env, lane, ws, 0u, 0u, 0u, obs16, stride16, false);
     else fx_step_repeat<STRATEGY, REWARD, V, false>(P, actions, obs, reward, reward64, terminated, env, lane, ws, 0u, 0u, 0u, nullptr, 0, false);
   } else {
@@ -1419,6 +1469,26 @@ fx_step_kernel(const __grid_constant__ FxKernelParams P, const void* __restrict_
 #ifdef FXENV_ENABLE_TIMING
   if (klog) { long long g2; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g2)); klog[3] = g2; }
 #endif
+}
+
+template <int STRATEGY, int REWARD, unsigned V>
+__global__ void __launch_bounds__(FX_WARPS * 32, FX_MIN_BLOCKS)
+fx_step_kernel(const __grid_constant__ FxKernelParams P, const void* __restrict__ actions, float* __restrict__ obs,
+               float* __restrict__ reward, double* __restrict__ reward64, uint8_t* __restrict__ terminated,
+               const int env_begin, const int env_end, uint16_t* __restrict__ obs16, const int stride16, const FxTileSync sync) {
+  fx_step_kernel_body<STRATEGY, REWARD, V, false>(P, actions, obs, reward, reward64, terminated, env_begin, env_end, obs16,
+                                                  stride16, sync, nullptr);
+}
+
+// The step kernel of a closed-loop rollout whose policy normalizes its observations (fxenv_policy_set_obs_norm)
+template <int STRATEGY, int REWARD, unsigned V>
+__global__ void __launch_bounds__(FX_WARPS * 32, FX_MIN_BLOCKS)
+fx_step_norm_kernel(const __grid_constant__ FxKernelParams P, const void* __restrict__ actions, float* __restrict__ obs,
+                    float* __restrict__ reward, double* __restrict__ reward64, uint8_t* __restrict__ terminated,
+                    const int env_begin, const int env_end, uint16_t* __restrict__ obs16, const int stride16,
+                    const FxTileSync sync, const __grid_constant__ FxObsNorm norm) {
+  fx_step_kernel_body<STRATEGY, REWARD, V, true>(P, actions, obs, reward, reward64, terminated, env_begin, env_end, obs16,
+                                                 stride16, sync, &norm);
 }
 
 // ---- K steps in ONE launch (fxenv_step_many): persistent warps pull (step chunk, env) tickets ----------------------
@@ -1519,9 +1589,10 @@ constexpr unsigned FX_V_HALF = FX_V_TRUNC | FX_V_PARAMS;
 template <unsigned HALF, int STRATEGY, int REWARD, unsigned V>
 FxEnvKernels fx_variant_entry() {
   if constexpr ((V & FX_V_HALF) == HALF && fx_variant_valid(STRATEGY, V))
-    return {fx_step_kernel<STRATEGY, REWARD, V & ~FX_V_RESIDENT>, fx_rollout_kernel<STRATEGY, REWARD, V>};
+    return {fx_step_kernel<STRATEGY, REWARD, V & ~FX_V_RESIDENT>, fx_rollout_kernel<STRATEGY, REWARD, V>,
+            fx_step_norm_kernel<STRATEGY, REWARD, V & ~FX_V_RESIDENT>};
   else
-    return {nullptr, nullptr};
+    return {nullptr, nullptr, nullptr};
 }
 
 template <unsigned HALF, size_t... I>

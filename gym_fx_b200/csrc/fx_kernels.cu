@@ -22,8 +22,11 @@ __global__ void fx_reset_kernel(const __grid_constant__ FxKernelParams P, const 
   fx_reset_env(P, env, start_bar ? start_bar[env] : st.start[env], start_bar == nullptr);
 }
 
-// writes the observation of the current state (what reset() returns): one warp per env
-__global__ void __launch_bounds__(FX_WARPS * 32) fx_observe_kernel(const __grid_constant__ FxKernelParams P, float* __restrict__ obs, uint16_t* __restrict__ obs16, const int stride16) {
+// writes the observation of the current state (what reset() returns): one warp per env.  NORM: the bf16 copy is the
+// normalized one of `norm` (fx_observe_norm_kernel; obs16 is then never nullptr).
+template <bool NORM>
+__device__ __forceinline__ void fx_observe_body(const FxKernelParams& P, float* __restrict__ obs, uint16_t* __restrict__ obs16,
+                                                const int stride16, const FxObsNorm* norm) {
   extern __shared__ __align__(16) unsigned char fx_smem[];
   const FxConfig& c = P.cfg;
   const FxDeviceState& st = P.st;
@@ -42,9 +45,25 @@ __global__ void __launch_bounds__(FX_WARPS * 32) fx_observe_kernel(const __grid_
   if (s < 1) s = 1;
   if (s > total_bars) s = total_bars;  // app/env.py:228
   float* row = obs + (int64_t)env * P.obs_dim;
-  uint16_t* row16 = obs16 ? obs16 + (int64_t)env * stride16 : nullptr;
-  if (lane == 0) fx_write_scalars(P, e, total_bars, tb.candles[(start + s - 1) * (int64_t)c.n_cols + c.price_col], row, row16);
-  fx_stream_windows<false>(P, tb, env, lane, s, start, ws, row, row16);
+  if constexpr (NORM) {
+    const FxRow16N row16 = fx_norm_row(*norm, obs16, stride16, env);
+    if (lane == 0) fx_write_scalars<false, FxRow16N>(P, e, total_bars, tb.candles[(start + s - 1) * (int64_t)c.n_cols + c.price_col], row, row16);
+    fx_stream_windows<false, FxRow16N>(P, tb, env, lane, s, start, ws, row, row16);
+  } else {
+    uint16_t* row16 = obs16 ? obs16 + (int64_t)env * stride16 : nullptr;
+    if (lane == 0) fx_write_scalars(P, e, total_bars, tb.candles[(start + s - 1) * (int64_t)c.n_cols + c.price_col], row, row16);
+    fx_stream_windows<false>(P, tb, env, lane, s, start, ws, row, row16);
+  }
+}
+
+__global__ void __launch_bounds__(FX_WARPS * 32) fx_observe_kernel(const __grid_constant__ FxKernelParams P, float* __restrict__ obs, uint16_t* __restrict__ obs16, const int stride16) {
+  fx_observe_body<false>(P, obs, obs16, stride16, nullptr);
+}
+
+__global__ void __launch_bounds__(FX_WARPS * 32)
+fx_observe_norm_kernel(const __grid_constant__ FxKernelParams P, float* __restrict__ obs, uint16_t* __restrict__ obs16,
+                       const int stride16, const __grid_constant__ FxObsNorm norm) {
+  fx_observe_body<true>(P, obs, obs16, stride16, &norm);
 }
 
 // Per-bar rolling z-score statistics (feature_window_preprocessor._scale_window :96-124 for a FULL window):
@@ -151,13 +170,18 @@ cudaError_t fx_configure_half(FxKernelParams& P, unsigned half) {
     if ((key & fixed) != want || !fx_variant_valid(P.cfg.strategy, key)) continue;
     const FxEnvKernels k = env_kernels(P, key);
     const FxStepKernelFn sk = k.step;
+    const FxStepNormKernelFn nk = k.step_norm;
     const FxRolloutKernelFn rk = k.rollout;
     cudaError_t e = cudaFuncSetAttribute(sk, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
+    if (e != cudaSuccess) return e;
+    e = cudaFuncSetAttribute(nk, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
     if (e != cudaSuccess) return e;
     e = cudaFuncSetAttribute(rk, cudaFuncAttributePreferredSharedMemoryCarveout, rpct);
     if (e != cudaSuccess) return e;
     if (smem > 48 * 1024) {
       e = cudaFuncSetAttribute(sk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      if (e != cudaSuccess) return e;
+      e = cudaFuncSetAttribute(nk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return e;
     }
     if (rsmem > 48 * 1024) {
@@ -190,7 +214,9 @@ cudaError_t fx_configure_kernels(FxKernelParams& P) {
   const cudaError_t e = fx_configure_half(P, 0u);
   if (e != cudaSuccess) return e;
   if (smem <= 48 * 1024) return cudaSuccess;
-  return cudaFuncSetAttribute(fx_observe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)observe_smem_bytes(P));
+  const cudaError_t e2 = cudaFuncSetAttribute(fx_observe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)observe_smem_bytes(P));
+  if (e2 != cudaSuccess) return e2;
+  return cudaFuncSetAttribute(fx_observe_norm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)observe_smem_bytes(P));
 }
 
 // The LEAN contract of the specialised kernels (see fx_uses_running_stats): everything here is a property of the
@@ -216,7 +242,7 @@ bool fx_config_is_lean(const FxKernelParams& P, const double* rows_host) {
 
 cudaError_t fx_launch_step(const FxKernelParams& P, const void* actions, float* obs, float* reward, double* reward64,
                            uint8_t* terminated, cudaStream_t stream, int env_begin, int env_end, uint16_t* obs16, int stride16,
-                           const FxTileSync* sync) {
+                           const FxTileSync* sync, const FxObsNorm* norm) {
   if (env_end < 0) env_end = P.cfg.num_envs;
   cudaLaunchConfig_t lc = {};
   lc.gridDim = dim3((env_end - env_begin + FX_WARPS - 1) / FX_WARPS);
@@ -229,6 +255,9 @@ cudaError_t fx_launch_step(const FxKernelParams& P, const void* actions, float* 
   lc.attrs = at;
   lc.numAttrs = (P.debug & 4) ? 0 : 1;  // FXENV_DEBUG & 4: plain stream-serialised launches (A/B timing only)
   const FxTileSync no_sync = {nullptr, nullptr, nullptr, 0};
+  if (norm && obs16)
+    return cudaLaunchKernelEx(&lc, env_kernels(P, fx_variant_key(P)).step_norm, P, actions, obs, reward, reward64, terminated,
+                              env_begin, env_end, obs16, stride16, sync ? *sync : no_sync, *norm);
   return cudaLaunchKernelEx(&lc, env_kernels(P, fx_variant_key(P)).step, P, actions, obs, reward, reward64, terminated, env_begin,
                             env_end, obs16, stride16, sync ? *sync : no_sync);
 }
@@ -302,9 +331,13 @@ cudaError_t fx_launch_reset(const FxKernelParams& P, const int64_t* start_bar, c
   return cudaGetLastError();
 }
 
-cudaError_t fx_launch_observe(const FxKernelParams& P, float* obs, cudaStream_t stream, uint16_t* obs16, int stride16) {
+cudaError_t fx_launch_observe(const FxKernelParams& P, float* obs, cudaStream_t stream, uint16_t* obs16, int stride16,
+                              const FxObsNorm* norm) {
   const int N = P.cfg.num_envs;
-  fx_observe_kernel<<<(N + FX_WARPS - 1) / FX_WARPS, FX_WARPS * 32, observe_smem_bytes(P), stream>>>(P, obs, obs16, stride16);
+  if (norm && obs16)
+    fx_observe_norm_kernel<<<(N + FX_WARPS - 1) / FX_WARPS, FX_WARPS * 32, observe_smem_bytes(P), stream>>>(P, obs, obs16, stride16, *norm);
+  else
+    fx_observe_kernel<<<(N + FX_WARPS - 1) / FX_WARPS, FX_WARPS * 32, observe_smem_bytes(P), stream>>>(P, obs, obs16, stride16);
   return cudaGetLastError();
 }
 

@@ -146,14 +146,33 @@ struct FxTileSync {
 #define FX_SYNC_TILE 128
 #define FX_SYNC_MAX_POLLS (1 << 22)   // x ~64 ns: a poll gives up after ~0.3 s instead of hanging the device  // obs16: optional bf16 copy of the rows
 
+// Observation normalizer of a closed-loop policy (fxenv_policy_set_obs_norm): every element the env kernels write to the
+// bf16 copy becomes bf16_rn(clamp((x - mean) * rstd, -clip, clip)) with the statistics of the env's population member
+// m = env / member_envs and pair p = env % num_pairs.  mean / rstd: float32 [members][num_pairs][stride16] (the bf16 row
+// stride, so that a row of statistics is 16-byte aligned wherever a row of the copy is 8-byte aligned); clip: [members].
+struct FxObsNorm {
+  const float* mean;
+  const float* rstd;
+  const float* clip;
+  int32_t member_envs;
+  int32_t num_pairs;
+};
+
+// norm (with obs16 only): the normalized variant of the bf16 copy -- separate kernels, so that the plain ones are unchanged
 cudaError_t fx_launch_step(const FxKernelParams& P, const void* actions, float* obs, float* reward, double* reward64,
                            uint8_t* terminated, cudaStream_t stream, int env_begin = 0, int env_end = -1,
-                           uint16_t* obs16 = nullptr, int stride16 = 0, const FxTileSync* sync = nullptr);
+                           uint16_t* obs16 = nullptr, int stride16 = 0, const FxTileSync* sync = nullptr,
+                           const FxObsNorm* norm = nullptr);
 
 cudaError_t fx_launch_reset(const FxKernelParams& P, const int64_t* start_bar, const uint8_t* mask, int first,
                             cudaStream_t stream);
 cudaError_t fx_launch_observe(const FxKernelParams& P, float* obs, cudaStream_t stream, uint16_t* obs16 = nullptr,
-                              int stride16 = 0);
+                              int stride16 = 0, const FxObsNorm* norm = nullptr);
+// Shifted column moments of rows [slots][num_envs][D] restricted to the envs [env_begin, env_end), by pair (env %
+// num_pairs): out[p][0][j] = sum (x - shift[p][j]), out[p][1][j] = sum (x - shift[p][j])^2, in float64, in an order fixed
+// by the shapes alone (fx_obs_stats.cu)
+cudaError_t fx_launch_obs_moments(const float* obs, int slots, int num_envs, int D, int num_pairs, int env_begin, int env_end,
+                                  const float* shift, double* out, cudaStream_t stream);
 cudaError_t fx_launch_stats(const FxConfig& cfg, const double* candles, double* stats, int64_t T, cudaStream_t stream);
 cudaError_t fx_configure_kernels(FxKernelParams& P);
 // the same for the kernel half `half` (its FX_V_TRUNC | FX_V_PARAMS bits, see below); the halves with either bit are
@@ -192,9 +211,12 @@ typedef void (*FxStepKernelFn)(const FxKernelParams, const void*, float*, float*
                                const FxTileSync);
 typedef void (*FxRolloutKernelFn)(const FxKernelParams, const char*, float*, int, float*, uint8_t*, const FxChunkPlan, unsigned,
                                   unsigned);
+typedef void (*FxStepNormKernelFn)(const FxKernelParams, const void*, float*, float*, double*, uint8_t*, int, int, uint16_t*,
+                                   int, const FxTileSync, const FxObsNorm);
 struct FxEnvKernels {
   FxStepKernelFn step;
   FxRolloutKernelFn rollout;
+  FxStepNormKernelFn step_norm;  // the step kernel with the normalized bf16 copy (fx_step_norm_kernel)
 };
 // The kernels are split over four translation units by the two bits FX_V_TRUNC and FX_V_PARAMS (the "half" of a key):
 // fx_kernels.cu holds the keys with neither, fx_kernels_trunc.cu those with FX_V_TRUNC only, fx_kernels_params.cu those

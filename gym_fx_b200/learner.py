@@ -14,6 +14,14 @@ With a time limit (VecFxEnv.set_time_limit) `done` holds codes: 1 = terminated, 
 the recursion and masks the reset step after it, but its TD target keeps gamma * V(final observation) -- value[t + 1],
 the value of the cut episode's last observation -- because the episode did not end in the MDP (Pardo et al., "Time
 Limits in Reinforcement Learning", 2018).
+
+Observation normalization (ActorCritic(obs_norm=True), an ObsNormalizer with running per-pair statistics, the
+counterpart of SB3's VecNormalize / CleanRL's NormalizeObservation).  The fused kernels normalize the bf16 copy the
+policy reads, where the float32 value still exists; the rollout's float32 obs stay raw.  One iteration, statistics k:
+    rollout with stats k (set_weights uploaded them)  ->  ppo_update (normalizes the raw obs with stats k, so the
+    probability ratio compares like with like)  ->  net.obs_norm.update(env, obs[:H])  ->  set_weights (weights and
+    stats k + 1)
+A population member updates its own normalizer from its env slice (envs=policy.member_envs(m)).
 """
 from __future__ import annotations
 
@@ -27,17 +35,95 @@ import torch.nn.functional as F
 from .sharding import allreduce_mean_grads
 
 
+class ObsNormalizer(nn.Module):
+    """Running mean / variance of the observation columns, per currency pair (env i trades pair i % num_pairs), applied
+    as y = clamp((x - mean) * rstd, -clip, clip) in float32, rstd = 1 / sqrt(var + eps) -- the formula and the float32
+    statistics the fused kernels apply to the policy's bf16 observation (include/fxenv.h fxenv_policy_set_obs_norm), so
+    forward() and the kernel agree bit for bit before the bf16 rounding.  A zero-variance column (the first return) maps
+    to 0.  Buffers mean / var float64 [P, D] and count float64 [P] go with state_dict; before the first update the
+    statistics are mean 0, var 1.  Batches merge by Chan et al.'s parallel algorithm from shifted sums (shift = the
+    float32 mean), which add up across ranks with one all-reduce."""
+
+    def __init__(self, obs_dim: int, num_pairs: int = 1, clip: float = 10.0, eps: float = 1e-8):
+        super().__init__()
+        if not clip > 0.0:
+            raise ValueError(f"clip must be > 0 (inf allowed), got {clip}")
+        self.obs_dim, self.num_pairs, self.clip, self.eps = int(obs_dim), int(num_pairs), float(clip), float(eps)
+        self.register_buffer("mean", torch.zeros(num_pairs, obs_dim, dtype=torch.float64))
+        self.register_buffer("var", torch.ones(num_pairs, obs_dim, dtype=torch.float64))
+        self.register_buffer("count", torch.zeros(num_pairs, dtype=torch.float64))
+
+    def mean32(self) -> torch.Tensor:
+        """float32 [P, D] mean: the shift of the moments and what forward() subtracts"""
+        return self.mean.float()
+
+    def rstd32(self) -> torch.Tensor:
+        """float32 [P, D] 1 / sqrt(var + eps), formed in float64"""
+        return (1.0 / torch.sqrt(self.var + self.eps)).float()
+
+    def forward(self, x: torch.Tensor, pair: torch.Tensor) -> torch.Tensor:
+        """x float32 [B, D], pair [B] (each row's pair index) -> the normalized rows, float32"""
+        return torch.clamp((x - self.mean32()[pair]) * self.rstd32()[pair], -self.clip, self.clip)
+
+    @torch.no_grad()
+    def update_from_moments(self, S: torch.Tensor, counts, dist=None):
+        """Merge a batch given by its shifted sums S float64 [P, 2, D] (S[p, 0] = sum (x - mean32[p]), S[p, 1] = sum of
+        the squares; VecFxEnv.obs_moments with shift=mean32()) over counts [P] rows per pair.  With torch.distributed
+        initialised, S and counts are summed over the ranks first (one all-reduce), so every rank ends with the same
+        statistics -- those of all ranks' rows."""
+        P, D = self.num_pairs, self.obs_dim
+        S = S.to(device=self.mean.device, dtype=torch.float64)
+        if tuple(S.shape) != (P, 2, D):
+            raise ValueError(f"S must have shape {(P, 2, D)}, got {tuple(S.shape)}")
+        n = torch.as_tensor(counts, dtype=torch.float64, device=self.mean.device).reshape(P)
+        if dist is not None and dist.is_initialized() and dist.get_world_size() > 1:
+            flat = torch.cat([S.reshape(-1), n])
+            dist.all_reduce(flat, op=dist.ReduceOp.SUM)
+            S, n = flat[:-P].view(P, 2, D), flat[-P:]
+        shift = self.mean32().double()
+        nb = n.clamp(min=1.0)[:, None]
+        mean_b = shift + S[:, 0] / nb
+        m2_b = torch.clamp(S[:, 1] - S[:, 0] * S[:, 0] / nb, min=0.0)
+        tot = self.count[:, None] + n[:, None]
+        delta = mean_b - self.mean
+        w = n[:, None] / tot.clamp(min=1.0)
+        mean = self.mean + delta * w
+        m2 = self.var * self.count[:, None] + m2_b + delta * delta * self.count[:, None] * w
+        var = m2 / tot.clamp(min=1.0)
+        has = (n > 0)[:, None]
+        self.mean.copy_(torch.where(has, mean, self.mean))
+        self.var.copy_(torch.where(has, var, self.var))
+        self.count.add_(n)
+
+    @torch.no_grad()
+    def update(self, env, obs: torch.Tensor, envs: slice = slice(None), dist=None):
+        """Merge rollout observations obs float32 [slots, N, D] (e.g. buf["obs"][:H]) of the envs `envs` (a contiguous
+        slice: a population member's policy.member_envs(m)) into the statistics, per pair, on the device
+        (VecFxEnv.obs_moments)."""
+        if env.cfg.num_pairs != self.num_pairs:
+            raise ValueError(f"the env has {env.cfg.num_pairs} pairs, the normalizer {self.num_pairs}")
+        obs = obs.contiguous()
+        e0, e1, _ = envs.indices(env.num_envs)
+        S = env.obs_moments(obs, self.mean32().to(env.device).contiguous(), slice(e0, e1))
+        P = self.num_pairs
+        per_pair = [len(range(e0 + (p - e0) % P, e1, P)) for p in range(P)]
+        self.update_from_moments(S, [c * int(obs.shape[0]) for c in per_pair], dist)
+
+
 class ActorCritic(nn.Module):
     """Shared-body actor-critic in the layout FusedPolicy.set_weights reads (body[0], body[2], pi, v).
     continuous=True (action_space_mode "continuous"): a Gaussian actor, `pi` = Linear(hidden, 1) gives the mean and the
     parameter `log_std` [1] the state-independent log sigma; forward() then returns (mean [B, 1], value).
     separate=True: separate actor and critic networks -- `body` feeds only `pi`, and `critic_body`, built like `body`,
     feeds `v`, so the value loss does not shape the policy's features (the layout of Stable-Baselines3's and CleanRL's
-    PPO).  The fused loop runs it as two networks (VecFxEnv.make_policy infers `separate` from the module)."""
+    PPO).  The fused loop runs it as two networks (VecFxEnv.make_policy infers `separate` from the module).
+    obs_norm=True: an ObsNormalizer(obs_dim, num_pairs) `obs_norm` normalizes the observation first (forward needs each
+    row's pair then); FusedPolicy.set_weights uploads its statistics with the weights."""
 
     def __init__(self, obs_dim: int, hidden: int = 256, n_actions: int = 3, continuous: bool = False,
-                 init_log_std: float = 0.0, separate: bool = False):
+                 init_log_std: float = 0.0, separate: bool = False, obs_norm: bool = False, num_pairs: int = 1):
         super().__init__()
+        self.obs_norm = ObsNormalizer(obs_dim, num_pairs) if obs_norm else None
         self.body = nn.Sequential(nn.Linear(obs_dim, hidden), nn.Tanh(), nn.Linear(hidden, hidden), nn.Tanh())
         self.pi = nn.Linear(hidden, 1 if continuous else n_actions)
         self.v = nn.Linear(hidden, 1)
@@ -48,7 +134,11 @@ class ActorCritic(nn.Module):
         if separate:
             self.critic_body = nn.Sequential(nn.Linear(obs_dim, hidden), nn.Tanh(), nn.Linear(hidden, hidden), nn.Tanh())
 
-    def forward(self, obs):
+    def forward(self, obs, pair=None):
+        if self.obs_norm is not None:
+            if pair is None:
+                raise ValueError("a normalizing ActorCritic needs each row's pair: forward(obs, pair)")
+            obs = self.obs_norm(obs, pair)
         h = self.body(obs)
         if self.separate:
             return self.pi(h), self.v(self.critic_body(obs)).squeeze(-1)
@@ -103,10 +193,12 @@ def masked_global_mean_std(x, mask, dist=None, eps: float = 1e-8):
 
 def ppo_update(net: ActorCritic, opt, buf: Dict[str, torch.Tensor], prev_done: torch.Tensor, dist=None, *, epochs: int = 1,
                minibatches: int = 4, clip: float = 0.2, vf_coef: float = 0.5, ent_coef: float = 0.01, max_grad_norm: float = 0.5,
-               gamma: float = 0.99, lam: float = 0.95, timers: Optional[dict] = None) -> Dict[str, float]:
+               gamma: float = 0.99, lam: float = 0.95, timers: Optional[dict] = None, env_offset: int = 0) -> Dict[str, float]:
     """One PPO update from a rollout buffer (VecFxEnv.rollout).  `timers`, if given, receives CUDA-event pairs around the
     collectives under "allreduce" so that the caller can report their share of the update.  Floating-point actions
-    (continuous action mode) are scored by the Gaussian actor of ActorCritic(continuous=True)."""
+    (continuous action mode) are scored by the Gaussian actor of ActorCritic(continuous=True).  A net with an
+    observation normalizer (net.obs_norm) gets each row's pair, (env_offset + env) % num_pairs: env_offset is the
+    handle's index of the buffer's first env (a population member's first env)."""
     obs, act, logp_old, val, rew, done = (buf[k] for k in ("obs", "actions", "logp", "value", "reward", "done"))
     H, N = rew.shape
     D = obs.shape[-1]
@@ -130,6 +222,8 @@ def ppo_update(net: ActorCritic, opt, buf: Dict[str, torch.Tensor], prev_done: t
     b_act, b_logp = (act.reshape(-1) if continuous else act.reshape(-1).long()), logp_old.reshape(-1)
     b_adv, b_ret, b_valid = adv.reshape(-1), ret.reshape(-1), valid.reshape(-1)
     params = [p for p in net.parameters()]
+    norm = getattr(net, "obs_norm", None)
+    b_pair = None if norm is None else ((env_offset + torch.arange(N, device=obs.device)) % norm.num_pairs).repeat(H)
     mb = (H * N) // minibatches
     stats = {}
     for _ in range(epochs):
@@ -138,7 +232,7 @@ def ppo_update(net: ActorCritic, opt, buf: Dict[str, torch.Tensor], prev_done: t
             idx = perm[k * mb:(k + 1) * mb]
             w = b_valid[idx]
             wn = w.sum().clamp(min=1.0)
-            logits, v = net(b_obs[idx])
+            logits, v = net(b_obs[idx]) if b_pair is None else net(b_obs[idx], b_pair[idx])
             if continuous:  # logits = the Gaussian mean [mb, 1]
                 new_logp = gaussian_log_prob(logits.squeeze(-1), net.log_std, b_act[idx])
             else:
@@ -176,4 +270,4 @@ def ppo_update_population(nets, opts, buf: Dict[str, torch.Tensor], prev_done: t
         raise ValueError(f"{N} envs do not split into {M} equal member slices")
     n = N // M
     return [ppo_update(nets[m], opts[m], {k: v[:, m * n:(m + 1) * n] for k, v in buf.items()},
-                       prev_done[m * n:(m + 1) * n], dist, **kw) for m in range(M)]
+                       prev_done[m * n:(m + 1) * n], dist, env_offset=m * n, **kw) for m in range(M)]

@@ -540,6 +540,26 @@ class VecFxEnv:
         policy._keep = (b, eps)
         return b
 
+    def obs_moments(self, obs: torch.Tensor, shift: torch.Tensor, envs: slice = slice(None)) -> torch.Tensor:
+        """Shifted column moments of rollout observations for an observation normalizer (include/fxenv.h
+        fxenv_obs_moments): obs float32 [slots, N, D] (a rollout's obs, or a prefix of it), shift float32 [num_pairs, D]
+        (the running mean).  Over every slot and the envs of `envs` (a contiguous slice, e.g. a population member's
+        policy.member_envs(m)), grouped by pair p = env % num_pairs: float64 [num_pairs, 2, D] with [p, 0] = sum (x -
+        shift[p]) and [p, 1] = sum (x - shift[p])^2.  The order of summation depends on the shapes only, so the same
+        inputs give the same bits.  Ordered on the current stream."""
+        P, N, D = int(self.cfg.num_pairs), self.num_envs, self.obs_dim
+        if not isinstance(obs, torch.Tensor) or obs.dim() != 3 or obs.shape[0] < 1:
+            raise ValueError(f"obs must be a [slots >= 1, {N}, {D}] tensor")
+        self._check("obs", obs, torch.float32, (int(obs.shape[0]), N, D))
+        self._check("shift", shift, torch.float32, (P, D))
+        if not isinstance(envs, slice) or envs.step not in (None, 1):
+            raise ValueError(f"envs must be a contiguous slice, got {envs!r}")
+        e0, e1, _ = envs.indices(N)
+        out = torch.empty((P, 2, D), dtype=torch.float64, device=self.device)
+        self._set("fxenv_obs_moments", obs.data_ptr(), int(obs.shape[0]), e0, e1, shift.data_ptr(), out.data_ptr(),
+                  self._stream())
+        return out
+
     def launch_count(self) -> int:
         return int(self.L.fxenv_launch_count(self._h))
 
@@ -612,7 +632,11 @@ class FusedPolicy:
     members (`self.members`, fixed too): a population of independent networks of that one width and layout (fxenv.h:
     fxenv_policy_create_ex3); member m acts for the envs `member_envs(m)` and gives there exactly what a single policy
     with its weights gives.  Weights come as a list or tuple of one module or dict per member (`set_weights`), or one
-    member at a time (`set_member_weights`); members whose weights disagree on the width or layout are a ValueError."""
+    member at a time (`set_member_weights`); members whose weights disagree on the width or layout are a ValueError.
+    Observation normalizer (fxenv.h: fxenv_policy_set_obs_norm): weights with one -- a module whose `obs_norm` is a
+    learner.ObsNormalizer (ActorCritic(obs_norm=True)), or a dict with obs_mean and obs_rstd float32 [num_pairs,
+    obs_dim] and obs_clip -- make the kernel normalize the bf16 observation it reads, with the statistics of each env's
+    pair; weights without one turn it off.  Every member has one or none."""
 
     HIDDEN = 256
     CRITIC_KEYS = ("w1_v", "b1_v", "w2_v", "b2_v")   # the critic trunk in a weight dict of a separate policy
@@ -657,6 +681,7 @@ class FusedPolicy:
         _native.check(env.L, env._h, rc, "fxenv_policy_create_ex3")
         self._keep = None
         self._w: Dict[int, Dict[str, torch.Tensor]] = {}
+        self._norm_on = [False] * members  # which members' weights came with an observation normalizer
         env._policies.append(self)
         if weights is not None:
             self.set_weights(weights)
@@ -725,19 +750,33 @@ class FusedPolicy:
         each = list(weights) if isinstance(weights, (list, tuple)) else [weights]
         if len(each) != self.members:
             raise ValueError(f"{len(each)} weight sets for a policy of {self.members} member(s)")
-        for m, ts in enumerate([self._tensors(w) for w in each]):
+        sets = [self._tensors(w) for w in each]
+        self._common(sets, lambda ts: "obs_mean" in ts, "observation normalizer (every member has one or none)")
+        for m, ts in enumerate(sets):
             self._upload(m, ts)
 
     def set_member_weights(self, m: int, weights):
         """New parameters for member m only (a module or weight dict of this policy's width and layout); the other
         members keep theirs, and the cached rollout graph stays."""
         self._check_member(m)
-        self._upload(int(m), self._tensors(weights))
+        ts = self._tensors(weights)
+        on = "obs_mean" in ts
+        others = [self._norm_on[k] for k in self._w if k != int(m)]
+        if any(o != on for o in others):
+            raise ValueError(f"member {m}'s weights {'have an' if on else 'have no'} observation normalizer, unlike the "
+                             "other members': every member has one or none")
+        self._upload(int(m), ts)
 
     def _upload(self, m: int, ts: Dict[str, torch.Tensor]):
         w = _native.FxPolicyWeights(*[ts[k].data_ptr() for k in ("w1", "b1", "w2", "b2", "w_pi", "b_pi", "w_v", "b_v")])
-        rc = self.env.L.fxenv_policy_set_member_weights(self._p, m, C.byref(w), self.env._stream())
-        _native.check(self.env.L, self.env._h, rc, "fxenv_policy_set_member_weights")
+        L, s = self.env.L, self.env._stream()
+        rc = L.fxenv_policy_set_member_weights(self._p, m, C.byref(w), s)
+        _native.check(L, self.env._h, rc, "fxenv_policy_set_member_weights")
+        on = "obs_mean" in ts
+        rc = L.fxenv_policy_set_obs_norm(self._p, m, ts["obs_mean"].data_ptr() if on else None,
+                                         ts["obs_rstd"].data_ptr() if on else None, float(ts["obs_clip"]) if on else 0.0, s)
+        _native.check(L, self.env._h, rc, "fxenv_policy_set_obs_norm")
+        self._norm_on[m] = on
         self._w[m] = ts  # keep the sources alive until the stream-ordered copies have run
 
     def _tensors(self, weights) -> Dict[str, torch.Tensor]:
@@ -757,6 +796,9 @@ class FusedPolicy:
                 if getattr(m, "log_std", None) is None:
                     raise ValueError("continuous action mode needs a log_std parameter of shape [1] on the module")
                 weights["log_std"] = m.log_std
+            nm = getattr(m, "obs_norm", None)
+            if nm is not None:  # learner.ObsNormalizer: the float32 statistics its forward() uses
+                weights.update({"obs_mean": nm.mean32(), "obs_rstd": nm.rstd32(), "obs_clip": nm.clip})
         D, Hd = self.env.obs_dim, self.hidden
         n_pi = 1 if self.continuous else 3
         shapes = {"w1": (Hd, D), "b1": (Hd,), "w2": (Hd, Hd), "b2": (Hd,), "w_pi": (n_pi, Hd), "b_pi": (n_pi,), "w_v": (Hd,),
@@ -781,6 +823,20 @@ class FusedPolicy:
         if self.separate:  # FxPolicyWeights under FXENV_POLICY_SEPARATE: both trunks stacked, the actor's first
             for k in ("w1", "b1", "w2", "b2"):
                 ts[k] = torch.cat([ts[k], ts.pop(k + "_v")])
+        given = [k for k in ("obs_mean", "obs_rstd", "obs_clip") if weights.get(k) is not None]
+        if given and len(given) != 3:
+            raise ValueError(f"an observation normalizer needs obs_mean, obs_rstd and obs_clip, got only {given}")
+        if given:
+            P = int(self.env.cfg.num_pairs)
+            for k in ("obs_mean", "obs_rstd"):
+                t = torch.as_tensor(weights[k]).detach().to(device=self.env.device, dtype=torch.float32).contiguous()
+                if tuple(t.shape) != (P, D):
+                    raise ValueError(f"{k} must have shape {(P, D)} (num_pairs, obs_dim), got {tuple(t.shape)}")
+                ts[k] = t
+            clip = float(weights["obs_clip"])
+            if not clip > 0.0:
+                raise ValueError(f"obs_clip must be > 0 (inf allowed), got {clip}")
+            ts["obs_clip"] = clip
         return ts
 
     def close(self):

@@ -23,6 +23,8 @@
  *   fxenv_set_action_repeat        (no counterpart: k bars per step, one decision per step; its contract below)
  *   fxenv_set_time_limit           (no counterpart: Gymnasium's max_episode_steps and truncation; its contract below)
  *   fxenv_set_env_params           (no counterpart: per-env commission / leverage / slippage / SL / TP; its contract below)
+ *   fxenv_policy_set_obs_norm      (no counterpart: the policy's running observation normalizer, SB3 VecNormalize /
+ *   fxenv_obs_moments               CleanRL NormalizeObservation; its contract below)
  *
  * Conventions: every function returns 0 on success, <0 on error (see FXENV_E_*); fxenv_last_error() gives the
  * message.  No exceptions or aborts cross the ABI.  The library owns env state (device struct-of-arrays) behind
@@ -507,9 +509,33 @@ int fxenv_rollout_ex(FxEnv* env, FxPolicy* pol, const FxRollout* io, uint32_t fl
  * results are invalid), or <0.  Synchronises the device. */
 int fxenv_policy_sync_timeouts(FxPolicy* pol);
 
+/* Observation normalizer of the policy.  The policy reads the observation in bfloat16; with a normalizer on, every
+ * element the env kernels write to that copy is
+ *     bf16_rn(min(max((x - mean[m][p][j]) * rstd[m][p][j], -clip[m]), clip[m]))
+ * each operation rounded in float32 (torch's clamp((x - mean) * rstd, -clip, clip) gives the same bits), x the float32
+ * value of the row, m = env / (num_envs / members) the env's member and p = env % num_pairs its pair.  The float32
+ * rows of FxRollout.obs, the env's outputs and state, and fxenv_step / fxenv_step_many do not change.
+ * Member `member`'s normalizer: mean_dev / rstd_dev float32 [num_pairs][obs_dim] DEVICE, copied stream-ordered into the
+ * policy; clip > 0 (+inf allowed); both NULL clears it.  A rollout needs every member on or every member off (mixed:
+ * FXENV_E_STATE).  Turning it on or off drops the cached rollout graph; a value update keeps it (like
+ * fxenv_policy_set_member_weights).  An invalid member, clip <= 0 or NaN, or only one of the two pointers NULL:
+ * FXENV_E_INVALID, and the policy stays as it was. */
+int fxenv_policy_set_obs_norm(FxPolicy* pol, int32_t member, const float* mean_dev, const float* rstd_dev, float clip,
+                              void* stream);
+/* The normalizer's statistics of rollout observations: obs_dev float32 [slots][num_envs][obs_dim] DEVICE (FxRollout.obs
+ * layout), over every slot and the envs [env_begin, env_end) (a member's slice, or all), grouped by pair p = env %
+ * num_pairs.  out_dev float64 [num_pairs][2][obs_dim] DEVICE receives S1 = sum (x - shift) and S2 = sum (x - shift)^2,
+ * the difference formed in float64 from float32 shift_dev [num_pairs][obs_dim] (the running mean: shifted sums of
+ * several ranks add up with one all-reduce SUM when every rank uses the same shift).  The summation order depends on
+ * the shapes only: the same inputs give the same bits.  Stream-ordered.  slots < 1 or a range outside [0, num_envs)
+ * or empty: FXENV_E_INVALID. */
+int fxenv_obs_moments(FxEnv* env, const float* obs_dev, int32_t slots, int32_t env_begin, int32_t env_end,
+                      const float* shift_dev, double* out_dev, void* stream);
+
 /* fxenv_policy_peek `what` */
 #define FXENV_PEEK_OBS16 0   /* slot 0 | 1: the bf16 observation copy the policy reads, [num_envs][k_pad] (k_pad = obs_dim
-                              * rounded up to a multiple of 64, zero pad columns); a rollout's step t reads slot t % 2 */
+                              * rounded up to a multiple of 64, zero pad columns); a rollout's step t reads slot t % 2.
+                              * With a normalizer on (fxenv_policy_set_obs_norm) it is the normalized copy. */
 #define FXENV_PEEK_H1 1      /* slot 0: the layer-1 activations of the last policy evaluation (after a rollout: the
                               * bootstrap one), bf16 [num_envs rounded up to a multiple of 128][hidden]; with
                               * FXENV_POLICY_SEPARATE [...][2 hidden]: the actor's columns, then the critic's */
