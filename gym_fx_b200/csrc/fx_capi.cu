@@ -822,6 +822,18 @@ int fxenv_debug_order_smem(int window_size, int n_cols, int ring_len, int order_
  * loaded; FXENV_NO_LEAN turns them off), 0 if the general ones, <0 on error. */
 int fxenv_debug_lean(const FxEnv* env) { return env ? env->P.lean : FXENV_E_INVALID; }
 
+/* debug / tests: the variant key (FX_V_* bits, fx_kernels.cuh) of the kernels the handle's next step, step-many or rollout
+ * launch runs (the step kernels ignore FX_V_RESIDENT), <0 on error. */
+int fxenv_debug_variant_key(const FxEnv* env) { return env ? (int)fx_debug_variant_key(env->P) : FXENV_E_INVALID; }
+
+/* debug / tests (no CUDA call): 1 if the library has a step, a step-norm and a rollout kernel for this strategy, reward
+ * and variant key, 0 if it has none, <0 for a strategy, reward or key out of range. */
+int fxenv_debug_variant_exists(int strategy, int reward, uint32_t key) {
+  if (strategy < 0 || strategy >= FX_N_STRATEGIES || reward < 0 || reward >= FX_N_REWARDS || key >= FX_V_KEYS)
+    return FXENV_E_INVALID;
+  return fx_debug_variant_exists(strategy, reward, key) ? 1 : 0;
+}
+
 /* debug (FXENV_TIMING=1): copies the [num_envs][FX_NSTAMP] phase stamps of the last step; returns FX_NSTAMP or <0 */
 int fxenv_debug_timings(FxEnv* env, long long* out_host) {
   if (!env || !out_host || !env->P.timing) return FXENV_E_STATE;

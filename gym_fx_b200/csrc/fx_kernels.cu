@@ -142,6 +142,18 @@ FxEnvKernels env_kernels(const FxKernelParams& P, unsigned key) {
 
 }  // namespace
 
+// tests (fxenv_debug_variant_key, fxenv_debug_variant_exists): the key a launch on P runs, and whether the lookup has
+// every kernel of a (strategy, reward, key)
+unsigned fx_debug_variant_key(const FxKernelParams& P) { return fx_variant_key(P); }
+
+bool fx_debug_variant_exists(int strategy, int reward, unsigned key) {
+  FxKernelParams P = {};
+  P.cfg.strategy = strategy;
+  P.cfg.reward = reward;
+  const FxEnvKernels k = env_kernels(P, key);
+  return k.step != nullptr && k.step_norm != nullptr && k.rollout != nullptr;
+}
+
 // The resident-table rollout kernel when its CTAs fit an SM as many warps as the global-table one runs (16): each
 // CTA at most 227 KB, and (16 / FX_ROLLOUT_WARPS(true)) CTAs plus their 1 KB reservations at most the SM's 228 KB.
 // force: 0 / 1 = FXENV_ORDER_SMEM (measurements, tests), < 0 = decide by the budget.

@@ -225,3 +225,7 @@ FxEnvKernels fx_trunc_kernels(int strategy, int reward, unsigned key);
 FxEnvKernels fx_params_kernels(int strategy, int reward, unsigned key);
 FxEnvKernels fx_params_trunc_kernels(int strategy, int reward, unsigned key);
 FxChunkPlan fx_rollout_plan(const FxKernelParams& P, int n_steps);  // the host's ticket accounting needs n_rounds
+// tests: fx_variant_key(P), and whether the lookup has a step, a step-norm and a rollout kernel for the triple
+// (strategy < FX_N_STRATEGIES, reward < FX_N_REWARDS, key < FX_V_KEYS)
+unsigned fx_debug_variant_key(const FxKernelParams& P);
+bool fx_debug_variant_exists(int strategy, int reward, unsigned key);
