@@ -17,6 +17,7 @@ minibatch and advantages are normalised with global statistics (gym_fx_b200.lear
     python examples/ppo_rollout.py --randomize-costs 1e-4,3e-4
     python examples/ppo_rollout.py --population 4 --eval-rollouts 2
     python examples/ppo_rollout.py --obs-norm --updates 5
+    python examples/ppo_rollout.py --reward-norm --updates 5
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 examples/ppo_rollout.py --envs 4096
 
 --action-space continuous trains a Gaussian actor on the Box(-1, 1) action (thresholded to hold / long / short by the
@@ -48,6 +49,11 @@ with --eval-rollouts, its greedy evaluation reward).  --envs must be a multiple 
 learner.ObsNormalizer): seeded from the observation reset() returns, updated from every rollout's observations after
 the PPO update (each member from its own envs), uploaded with the weights; the fused kernels apply them to the bf16
 copy the policy reads.  obs_norm_update_s: the time of one statistics update.
+--reward-norm scales the rewards GAE reads by the running standard deviation of the discounted return and clips them
+to +-(--reward-clip) (learner.RewardNormalizer, gamma = PPO's): each member's normalizer scans its own envs' returns on
+the device after every rollout, and that update's scale applies to the same rollout.  reward_norm_std: sqrt(var) of the
+normalizer (a list, one per member, for a population); reward_norm_update_s: the time of one statistics update.  The
+reported and evaluation rewards stay raw.
 Prints one JSON line: env-steps/s (decisions) of the rollout phase (policy in the loop) and of the whole train loop, and
 bars/s of the rollout phase as an upper bound (decisions x K: a step that ends an episode runs fewer bars).
 """
@@ -55,6 +61,7 @@ from __future__ import annotations
 
 import argparse
 import json
+import math
 import os
 import sys
 import time
@@ -99,6 +106,9 @@ def main():
     ap.add_argument("--seed", type=int, default=0, help="parameter seed (member m of a population: seed + m)")
     ap.add_argument("--obs-norm", action="store_true",
                     help="normalize the policy's observations with running per-pair mean / variance statistics")
+    ap.add_argument("--reward-norm", action="store_true",
+                    help="scale rewards by the running standard deviation of the discounted return before GAE")
+    ap.add_argument("--reward-clip", type=float, default=10.0, help="clip of the scaled rewards (with --reward-norm)")
     args = ap.parse_args()
     continuous = args.action_space == "continuous"
     cost_max = None
@@ -120,9 +130,11 @@ def main():
     M = args.population
     if M < 1 or args.envs % (128 * M):
         ap.error("--population must be >= 1, and --envs a multiple of 128 x --population")
+    if not args.reward_clip > 0.0:
+        ap.error("--reward-clip must be > 0")
 
     import bench
-    from gym_fx_b200.learner import ActorCritic, ppo_update, ppo_update_population
+    from gym_fx_b200.learner import ActorCritic, RewardNormalizer, ppo_update, ppo_update_population
     from gym_fx_b200.sharding import check_pair_alignment, shard_starts
     from gym_fx_b200.vec_env import VecFxEnv
 
@@ -193,11 +205,15 @@ def main():
         desc += ", obs-norm (running per-pair statistics)"
         for m in range(M):
             nets[m].obs_norm.update(env, env.obs[None], envs=member_envs[m], dist=dist)
+    rnorms = None
+    if args.reward_norm:   # gamma: ppo_update's default, the discount of the returns GAE forms
+        desc += f", reward-norm (clip {args.reward_clip:g})"
+        rnorms = [RewardNormalizer(N // M, clip=args.reward_clip).to(dev) for _ in range(M)]
     policy = env.make_policy(nets if M > 1 else net)
     buf = None
     prev_done = torch.zeros(N, dtype=torch.uint8, device=dev)
 
-    t_roll = t_upd = t_norm = 0.0
+    t_roll = t_upd = t_norm = t_rnorm = 0.0
     stats = {}
     member_stats = [{} for _ in range(M)]   # a population: the last update's stats of each member
     cost_rng = np.random.default_rng(0xC057 + rank) if cost_max else None
@@ -212,12 +228,19 @@ def main():
         buf = env.rollout(policy, H, buffers=buf, seed=1000 * rank + it)
         torch.cuda.synchronize(dev)
         t1 = time.perf_counter()
+        if rnorms:   # this rollout's returns first, so that the update scales with statistics that include them
+            for m in range(M):
+                rnorms[m].update(env, buf, prev_done, envs=member_envs[m], dist=dist)
+            torch.cuda.synchronize(dev)
+            if it > 0:
+                t_rnorm += time.perf_counter() - t1
         if M > 1:
             member_stats = ppo_update_population(nets, opts, buf, prev_done, dist, epochs=args.epochs,
-                                                 minibatches=args.minibatches)
+                                                 minibatches=args.minibatches, reward_norms=rnorms)
             stats = {}
         else:
-            stats = ppo_update(net, opt, buf, prev_done, dist, epochs=args.epochs, minibatches=args.minibatches)
+            stats = ppo_update(net, opt, buf, prev_done, dist, epochs=args.epochs, minibatches=args.minibatches,
+                               reward_norm=rnorms[0] if rnorms else None)
         prev_done = buf["done"][-1].clone()
         if args.obs_norm:   # after the update, which normalized with the statistics the rollout used
             torch.cuda.synchronize(dev)
@@ -302,7 +325,10 @@ def main():
             "train_env_steps_per_s": steps / max(t_roll + t_upd, 1e-9), "update_s": t_upd / n_it,
             "obs_norm": args.obs_norm, "obs_norm_update_s": t_norm / n_it if args.obs_norm else None,
             "obs_norm_finite": all(bool(torch.isfinite(n.obs_norm.mean).all() and torch.isfinite(n.obs_norm.var).all())
-                                   for n in nets) if args.obs_norm else None, **stats,
+                                   for n in nets) if args.obs_norm else None,
+            "reward_norm": args.reward_norm, "reward_norm_update_s": t_rnorm / n_it if rnorms else None,
+            "reward_norm_std": (None if not rnorms else [math.sqrt(float(r.var)) for r in rnorms] if M > 1
+                                else math.sqrt(float(rnorms[0].var))), **stats,
             **({"members": members} if M > 1 else {})}), flush=True)
     env.close()
     if dist:

@@ -34,6 +34,7 @@ EXPORTS = [
     "fxenv_set_bracket_audit", "fxenv_get_bracket_audit", "fxenv_set_action_repeat", "fxenv_policy_create_ex",
     "fxenv_set_time_limit", "fxenv_set_env_params", "fxenv_policy_create_ex2", "fxenv_policy_create_ex3",
     "fxenv_policy_set_member_weights", "fxenv_policy_set_obs_norm", "fxenv_obs_moments",
+    "fxenv_return_moments",
 ]
 
 ROLLOUT_GREEDY = 1  # FXENV_ROLLOUT_GREEDY
@@ -90,8 +91,8 @@ INFO_DTYPES = {
 def build(force: bool = False, verbose: bool = False) -> str:
     """Compile gym_fx_b200/csrc/*.cu into gym_fx_b200/libfxenv.so with nvcc for sm_90a (works without a GPU)."""
     srcs = [os.path.join(CSRC, f) for f in ("fx_capi.cu", "fx_kernels.cu", "fx_kernels_trunc.cu", "fx_kernels_params.cu",
-                                            "fx_kernels_params_trunc.cu", "fx_policy.cu", "fx_obs_stats.cu", "fx_core.cuh",
-                                            "fx_kernels.cuh", "fx_env_step.cuh", "fx_policy.cuh", "Makefile")]
+                                            "fx_kernels_params_trunc.cu", "fx_policy.cu", "fx_obs_stats.cu", "fx_return_stats.cu",
+                                            "fx_core.cuh", "fx_kernels.cuh", "fx_env_step.cuh", "fx_policy.cuh", "Makefile")]
     srcs.append(os.path.join(_HERE, "..", "include", "fxenv.h"))
     stale = (not os.path.exists(LIB_PATH)) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in srcs)
     if force or stale:
@@ -160,6 +161,8 @@ def load():
     L.fxenv_set_env_params.argtypes = [vp, vp]
     L.fxenv_policy_set_obs_norm.argtypes = [vp, C.c_int32, vp, vp, C.c_float, vp]
     L.fxenv_obs_moments.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, vp, vp, vp]
+    L.fxenv_return_moments.argtypes = [vp, vp, vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double, vp, vp,
+                                       vp, vp]
     if L.fxenv_abi_version() != 2:
         raise FxEnvError("libfxenv.so ABI version mismatch")
     _lib = L

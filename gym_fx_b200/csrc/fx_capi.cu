@@ -1195,6 +1195,29 @@ int fxenv_obs_moments(FxEnv* env, const float* obs_dev, int32_t slots, int32_t e
   return FXENV_OK;
 }
 
+int fxenv_return_moments(FxEnv* env, const float* reward_dev, const uint8_t* done_dev, const uint8_t* prev_done_dev,
+                         int32_t horizon, int32_t env_begin, int32_t env_end, double gamma, double shift,
+                         double* ret_dev, int32_t* seen_dev, double* out_dev, void* stream_) {
+  if (!env) return FXENV_E_INVALID;
+  if (!reward_dev || !done_dev || !prev_done_dev || !ret_dev || !seen_dev || !out_dev)
+    return fail(env, FXENV_E_INVALID, "fxenv_return_moments: null pointer");
+  const int N = env->P.cfg.num_envs;
+  if (horizon < 1)
+    return fail(env, FXENV_E_INVALID, "fxenv_return_moments: horizon must be >= 1, got " + std::to_string(horizon));
+  if (env_begin < 0 || env_end > N || env_begin >= env_end)
+    return fail(env, FXENV_E_INVALID, "fxenv_return_moments: env range [" + std::to_string(env_begin) + ", " +
+                                      std::to_string(env_end) + ") is empty or outside [0, " + std::to_string(N) + ")");
+  if (!(gamma >= 0.0 && gamma <= 1.0))  // also NaN
+    return fail(env, FXENV_E_INVALID, "fxenv_return_moments: gamma must be in [0, 1], got " + std::to_string(gamma));
+  if (!isfinite(shift))
+    return fail(env, FXENV_E_INVALID, "fxenv_return_moments: shift must be finite, got " + std::to_string(shift));
+  DeviceGuard g(env->device);
+  FX_CUDA(env, fx_launch_return_moments(reward_dev, done_dev, prev_done_dev, env->P.st.ep_begun, N, horizon, env_begin,
+                                        env_end, gamma, shift, ret_dev, seen_dev, out_dev, (cudaStream_t)stream_));
+  env->launches += 2;
+  return FXENV_OK;
+}
+
 int fxenv_rollout(FxEnv* env, FxPolicy* pol, const FxRollout* io, void* stream_) {
   return fxenv_rollout_ex(env, pol, io, 0u, stream_);
 }

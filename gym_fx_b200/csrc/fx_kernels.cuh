@@ -173,6 +173,13 @@ cudaError_t fx_launch_observe(const FxKernelParams& P, float* obs, cudaStream_t 
 // by the shapes alone (fx_obs_stats.cu)
 cudaError_t fx_launch_obs_moments(const float* obs, int slots, int num_envs, int D, int num_pairs, int env_begin, int env_end,
                                   const float* shift, double* out, cudaStream_t stream);
+// Moments of the discounted returns of a rollout's rewards for the envs [env_begin, env_end), carried across calls in
+// ret / seen and cleared by any episode begun outside the rollout's reset steps (begun = FxDeviceState::ep_begun):
+// out = {sum (R - shift), sum (R - shift)^2, count} in float64, in an order fixed by the shapes alone (fx_return_stats.cu)
+cudaError_t fx_launch_return_moments(const float* reward, const uint8_t* done, const uint8_t* prev_done,
+                                     const int32_t* begun, int num_envs, int horizon, int env_begin, int env_end,
+                                     double gamma, double shift, double* ret, int32_t* seen, double* out,
+                                     cudaStream_t stream);
 cudaError_t fx_launch_stats(const FxConfig& cfg, const double* candles, double* stats, int64_t T, cudaStream_t stream);
 cudaError_t fx_configure_kernels(FxKernelParams& P);
 // the same for the kernel half `half` (its FX_V_TRUNC | FX_V_PARAMS bits, see below); the halves with either bit are

@@ -22,6 +22,14 @@ policy reads, where the float32 value still exists; the rollout's float32 obs st
     probability ratio compares like with like)  ->  net.obs_norm.update(env, obs[:H])  ->  set_weights (weights and
     stats k + 1)
 A population member updates its own normalizer from its env slice (envs=policy.member_envs(m)).
+
+Reward normalization (RewardNormalizer, the counterpart of SB3's VecNormalize(norm_reward=True) / gymnasium's
+NormalizeReward): rewards divided by the running standard deviation of the discounted return and clipped, so that the
+critic's targets sit near O(1) whatever the reward plugin, reward_scale, costs or leverage.  The returns are scanned on
+the device (VecFxEnv.return_moments), carried per env across rollouts.  One iteration, as in SB3:
+    rollout  ->  reward_norm.update(env, buf, prev_done) with this rollout's returns  ->  ppo_update(...,
+    reward_norm=reward_norm) (GAE reads the rewards scaled with the updated statistics; the buffer stays raw)
+A population member has its own normalizer on its own env slice.
 """
 from __future__ import annotations
 
@@ -110,6 +118,84 @@ class ObsNormalizer(nn.Module):
         self.update_from_moments(S, [c * int(obs.shape[0]) for c in per_pair], dist)
 
 
+class RewardNormalizer(nn.Module):
+    """Reward scaling by the running standard deviation of the discounted return, per env slice (one per population
+    member): the counterpart of SB3's VecNormalize(norm_reward=True) / gymnasium's NormalizeReward, with CleanRL's
+    reward clip.  normalize(r) = clamp(r * float32(1 / sqrt(var + eps)), -clip, clip); the mean is not subtracted.
+    Buffers, all in state_dict: mean / var / count float64 [1] (0, 1, 0 before the first update) -- the statistics of
+    the returns R_t = gamma R_{t-1} + r_t of every scanned step -- and ret float64 [num_envs] / seen int32 [num_envs]
+    (zeros / -1), each env's return carried from one rollout to the next (VecFxEnv.return_moments: cut at every done,
+    cleared when the env began an episode outside the scanned rollouts).  Batches merge by Chan et al.'s parallel
+    algorithm from shifted sums, which add up across ranks with one all-reduce."""
+
+    def __init__(self, num_envs: int, gamma: float = 0.99, clip: float = 10.0, eps: float = 1e-8):
+        super().__init__()
+        if isinstance(num_envs, bool) or int(num_envs) != num_envs or num_envs < 1:
+            raise ValueError(f"num_envs must be a positive integer, got {num_envs!r}")
+        if not 0.0 <= gamma <= 1.0:
+            raise ValueError(f"gamma must be in [0, 1], got {gamma}")
+        if not clip > 0.0:
+            raise ValueError(f"clip must be > 0 (inf allowed), got {clip}")
+        if not 0.0 < eps < math.inf:
+            raise ValueError(f"eps must be finite and > 0, got {eps}")
+        self.num_envs, self.gamma, self.clip, self.eps = int(num_envs), float(gamma), float(clip), float(eps)
+        self.register_buffer("mean", torch.zeros(1, dtype=torch.float64))
+        self.register_buffer("var", torch.ones(1, dtype=torch.float64))
+        self.register_buffer("count", torch.zeros(1, dtype=torch.float64))
+        self.register_buffer("ret", torch.zeros(self.num_envs, dtype=torch.float64))
+        self.register_buffer("seen", torch.full((self.num_envs,), -1, dtype=torch.int32))
+
+    def scale32(self) -> torch.Tensor:
+        """float32 [1] 1 / sqrt(var + eps), formed in float64"""
+        return (1.0 / torch.sqrt(self.var + self.eps)).float()
+
+    def normalize(self, reward: torch.Tensor) -> torch.Tensor:
+        """the scaled, clipped float32 rewards (any shape)"""
+        return torch.clamp(reward * self.scale32(), -self.clip, self.clip)
+
+    @torch.no_grad()
+    def update_from_moments(self, S: torch.Tensor, dist=None, shift=None):
+        """Merge a batch of returns given by its sums S float64 [3] = (sum (R - shift), sum (R - shift)^2, count);
+        shift None means the running mean.  With torch.distributed initialised, S is summed over the ranks first (one
+        all-reduce), so every rank ends with the same statistics -- those of all ranks' returns."""
+        S = S.to(device=self.mean.device, dtype=torch.float64).reshape(-1)
+        if S.numel() != 3:
+            raise ValueError(f"S must have 3 elements, got {S.numel()}")
+        if dist is not None and dist.is_initialized() and dist.get_world_size() > 1:
+            S = S.clone()
+            dist.all_reduce(S, op=dist.ReduceOp.SUM)
+        s1, s2, n = S[0:1], S[1:2], S[2:3]
+        base = self.mean if shift is None else torch.full_like(self.mean, float(shift))
+        nb = n.clamp(min=1.0)
+        mean_b = base + s1 / nb
+        m2_b = torch.clamp(s2 - s1 * s1 / nb, min=0.0)
+        tot = self.count + n
+        delta = mean_b - self.mean
+        w = n / tot.clamp(min=1.0)
+        mean = self.mean + delta * w
+        m2 = self.var * self.count + m2_b + delta * delta * self.count * w
+        var = m2 / tot.clamp(min=1.0)
+        has = n > 0
+        self.mean.copy_(torch.where(has, mean, self.mean))
+        self.var.copy_(torch.where(has, var, self.var))
+        self.count.add_(n)
+
+    @torch.no_grad()
+    def update(self, env, buf: Dict[str, torch.Tensor], prev_done: torch.Tensor, envs: slice = slice(None), dist=None):
+        """Merge the returns of a rollout buffer (VecFxEnv.rollout: its reward and done) of the envs `envs` (a contiguous
+        slice of num_envs envs, e.g. a population member's policy.member_envs(m)) into the statistics, on the device and
+        without a host synchronisation.  prev_done uint8 [N]: the done of the step before the rollout.  The scan's shift is
+        0, not the running mean, because the mean lives on the device and the host would have to wait to read it; in
+        float64 the unshifted sums lose about log10(mean^2 / var) of their 16 digits, nothing at the scale of returns."""
+        if not isinstance(envs, slice) or envs.step not in (None, 1):
+            raise ValueError(f"envs must be a contiguous slice, got {envs!r}")
+        e0, e1, _ = envs.indices(env.num_envs)
+        if e1 - e0 != self.num_envs:
+            raise ValueError(f"the slice has {max(e1 - e0, 0)} envs, the normalizer {self.num_envs}")
+        S = env.return_moments(buf["reward"], buf["done"], prev_done, self.ret, self.seen, self.gamma, 0.0, slice(e0, e1))
+        self.update_from_moments(S, dist, shift=0.0)
+
+
 class ActorCritic(nn.Module):
     """Shared-body actor-critic in the layout FusedPolicy.set_weights reads (body[0], body[2], pi, v).
     continuous=True (action_space_mode "continuous"): a Gaussian actor, `pi` = Linear(hidden, 1) gives the mean and the
@@ -193,12 +279,14 @@ def masked_global_mean_std(x, mask, dist=None, eps: float = 1e-8):
 
 def ppo_update(net: ActorCritic, opt, buf: Dict[str, torch.Tensor], prev_done: torch.Tensor, dist=None, *, epochs: int = 1,
                minibatches: int = 4, clip: float = 0.2, vf_coef: float = 0.5, ent_coef: float = 0.01, max_grad_norm: float = 0.5,
-               gamma: float = 0.99, lam: float = 0.95, timers: Optional[dict] = None, env_offset: int = 0) -> Dict[str, float]:
+               gamma: float = 0.99, lam: float = 0.95, timers: Optional[dict] = None, env_offset: int = 0,
+               reward_norm: Optional[RewardNormalizer] = None) -> Dict[str, float]:
     """One PPO update from a rollout buffer (VecFxEnv.rollout).  `timers`, if given, receives CUDA-event pairs around the
     collectives under "allreduce" so that the caller can report their share of the update.  Floating-point actions
     (continuous action mode) are scored by the Gaussian actor of ActorCritic(continuous=True).  A net with an
     observation normalizer (net.obs_norm) gets each row's pair, (env_offset + env) % num_pairs: env_offset is the
-    handle's index of the buffer's first env (a population member's first env)."""
+    handle's index of the buffer's first env (a population member's first env).  reward_norm: GAE reads
+    reward_norm.normalize(buf["reward"]) instead of the raw rewards (the buffer and the statistics stay as they are)."""
     obs, act, logp_old, val, rew, done = (buf[k] for k in ("obs", "actions", "logp", "value", "reward", "done"))
     H, N = rew.shape
     D = obs.shape[-1]
@@ -215,6 +303,8 @@ def ppo_update(net: ActorCritic, opt, buf: Dict[str, torch.Tensor], prev_done: t
         return out
 
     with torch.no_grad():
+        if reward_norm is not None:
+            rew = reward_norm.normalize(rew)
         adv, ret, valid = gae(rew, val, done, prev_done, gamma, lam)
         m, s = timed(lambda: masked_global_mean_std(adv, valid, dist))
         adv = (adv - m) / s
@@ -257,17 +347,21 @@ def ppo_update(net: ActorCritic, opt, buf: Dict[str, torch.Tensor], prev_done: t
 
 
 def ppo_update_population(nets, opts, buf: Dict[str, torch.Tensor], prev_done: torch.Tensor, dist=None,
-                          **kw) -> List[Dict[str, float]]:
+                          reward_norms=None, **kw) -> List[Dict[str, float]]:
     """One PPO update of every member of a policy population (VecFxEnv.make_policy(members=M)) from one rollout buffer:
     ppo_update(nets[m], opts[m], ...) on member m's envs, the contiguous slice [m N / M, (m + 1) N / M) of every
     buffer's env axis and of prev_done, members in order.  Each member's advantages are normalised over its own envs
-    on all ranks.  kw: ppo_update's keyword arguments.  Returns one stats dict per member."""
+    on all ranks.  reward_norms: one RewardNormalizer per member (built for N / M envs), or None.  kw: ppo_update's
+    keyword arguments.  Returns one stats dict per member."""
     M = len(nets)
     if M < 1 or len(opts) != M:
         raise ValueError(f"{M} networks and {len(opts)} optimisers: one optimiser per member")
+    if reward_norms is not None and len(reward_norms) != M:
+        raise ValueError(f"{len(reward_norms)} reward normalizers for {M} members: one per member")
     N = int(buf["reward"].shape[1])
     if N % M:
         raise ValueError(f"{N} envs do not split into {M} equal member slices")
     n = N // M
     return [ppo_update(nets[m], opts[m], {k: v[:, m * n:(m + 1) * n] for k, v in buf.items()},
-                       prev_done[m * n:(m + 1) * n], dist, env_offset=m * n, **kw) for m in range(M)]
+                       prev_done[m * n:(m + 1) * n], dist, env_offset=m * n,
+                       reward_norm=None if reward_norms is None else reward_norms[m], **kw) for m in range(M)]

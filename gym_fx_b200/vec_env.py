@@ -560,6 +560,34 @@ class VecFxEnv:
                   self._stream())
         return out
 
+    def return_moments(self, reward: torch.Tensor, done: torch.Tensor, prev_done: torch.Tensor, ret: torch.Tensor,
+                       seen: torch.Tensor, gamma: float, shift: float, envs: slice = slice(None)) -> torch.Tensor:
+        """Moments of the discounted returns of a rollout for a reward normalizer (include/fxenv.h
+        fxenv_return_moments): reward float32 [H, N] and done uint8 [H, N] (a rollout's buffers), prev_done uint8 [N] (the
+        done of the step before it).  Over the envs of `envs` (a contiguous slice, e.g. a population member's
+        policy.member_envs(m)), whose returns carry over from call to call in ret float64 [W] and seen int32 [W] (W = the
+        slice's width; start from zeros and -1), updated in place.  Reset steps are skipped, any done ends the return,
+        and an episode begun outside this rollout's reset steps clears it.  Returns float64 [3] = (sum (R - shift),
+        sum (R - shift)^2, count) over the slice's scanned steps, in an order that depends on the shapes only.  Ordered on
+        the current stream."""
+        N = self.num_envs
+        if not isinstance(reward, torch.Tensor) or reward.dim() != 2 or reward.shape[0] < 1:
+            raise ValueError(f"reward must be a [H >= 1, {N}] tensor")
+        H = int(reward.shape[0])
+        self._check("reward", reward, torch.float32, (H, N))
+        self._check("done", done, torch.uint8, (H, N))
+        self._check("prev_done", prev_done, torch.uint8, (N,))
+        if not isinstance(envs, slice) or envs.step not in (None, 1):
+            raise ValueError(f"envs must be a contiguous slice, got {envs!r}")
+        e0, e1, _ = envs.indices(N)
+        W = max(e1 - e0, 0)
+        self._check("ret", ret, torch.float64, (W,))
+        self._check("seen", seen, torch.int32, (W,))
+        out = torch.empty(3, dtype=torch.float64, device=self.device)
+        self._set("fxenv_return_moments", reward.data_ptr(), done.data_ptr(), prev_done.data_ptr(), H, e0, e1,
+                  float(gamma), float(shift), ret.data_ptr(), seen.data_ptr(), out.data_ptr(), self._stream())
+        return out
+
     def launch_count(self) -> int:
         return int(self.L.fxenv_launch_count(self._h))
 

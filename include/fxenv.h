@@ -25,6 +25,8 @@
  *   fxenv_set_env_params           (no counterpart: per-env commission / leverage / slippage / SL / TP; its contract below)
  *   fxenv_policy_set_obs_norm      (no counterpart: the policy's running observation normalizer, SB3 VecNormalize /
  *   fxenv_obs_moments               CleanRL NormalizeObservation; its contract below)
+ *   fxenv_return_moments           (no counterpart: SB3 VecNormalize(norm_reward), gymnasium NormalizeReward; its contract
+ *                                   below)
  *
  * Conventions: every function returns 0 on success, <0 on error (see FXENV_E_*); fxenv_last_error() gives the
  * message.  No exceptions or aborts cross the ABI.  The library owns env state (device struct-of-arrays) behind
@@ -531,6 +533,28 @@ int fxenv_policy_set_obs_norm(FxPolicy* pol, int32_t member, const float* mean_d
  * or empty: FXENV_E_INVALID. */
 int fxenv_obs_moments(FxEnv* env, const float* obs_dev, int32_t slots, int32_t env_begin, int32_t env_end,
                       const float* shift_dev, double* out_dev, void* stream);
+/* The reward normalizer's statistics: moments of the discounted return of every env, carried across rollouts.
+ * reward_dev float32 [horizon][num_envs], done_dev uint8 [horizon][num_envs] (FxRollout.reward / done: 0, or 1 / 2 =
+ * terminated / truncated), prev_done_dev uint8 [num_envs] (the done of the step before the rollout), all DEVICE.  Over
+ * the envs [env_begin, env_end) (a member's slice, or all); ret_dev float64 and seen_dev int32 DEVICE, env_end -
+ * env_begin entries each, env i at [i - env_begin], read and written.  For each env, with begun = the episodes the env
+ * has begun since fxenv_create (every reset, auto or explicit, counts; snapshots carry it):
+ *   reset(t) = t == 0 ? prev_done[i] != 0 : done[t-1][i] != 0      (the learner's reset steps)
+ *   R = begun - (number of t with reset(t)) == seen ? ret : 0       (any other reset since the last scan clears it)
+ *   for t in 0 .. horizon-1:  if !reset(t): R = R * gamma + (double)reward[t][i] (two roundings), d = R - shift,
+ *                             S1 += d, S2 += d * d, n += 1;  if done[t][i] != 0: R = 0  (termination and truncation)
+ *   ret = R, seen = begun
+ * out_dev float64 [3] DEVICE receives {S1, S2, n} summed over the slice (shifted sums of several ranks add up with one
+ * all-reduce SUM when every rank uses the same shift).  Start with ret = 0 and seen = -1.  Rewards of steps that no call
+ * scanned (fxenv_step_many, greedy rollouts) do not enter the return; an episode that ended or was reset in between still
+ * clears it, through begun.  A fxenv_set_state that rewinds an env past one of its resets clears it the same way; one
+ * that does not keeps the carried return.  The summation order depends only on (horizon, env_begin, env_end): the same
+ * inputs give the same bits; no atomics.  Stream-ordered, no host synchronisation.  horizon < 1, a range outside
+ * [0, num_envs) or empty, gamma outside [0, 1] or NaN, a non-finite shift or a NULL pointer: FXENV_E_INVALID, nothing
+ * enqueued. */
+int fxenv_return_moments(FxEnv* env, const float* reward_dev, const uint8_t* done_dev, const uint8_t* prev_done_dev,
+                         int32_t horizon, int32_t env_begin, int32_t env_end, double gamma, double shift,
+                         double* ret_dev, int32_t* seen_dev, double* out_dev, void* stream);
 
 /* fxenv_policy_peek `what` */
 #define FXENV_PEEK_OBS16 0   /* slot 0 | 1: the bf16 observation copy the policy reads, [num_envs][k_pad] (k_pad = obs_dim
